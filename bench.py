@@ -48,26 +48,13 @@ ALGO_BYTES = {
 }
 
 
-def ncu_traffic(kernel, streams):
-    """DRAM bytes per launch of `kernel` from the committed ncu capture (profiles/ncu_traffic.json), or None."""
-    p = os.path.join(ROOT, "profiles", "ncu_traffic.json")
-    try:
-        with open(p) as f:
-            d = json.load(f)
-        if d.get("streams") == streams and kernel in d:
-            return d[kernel]
-    except (OSError, ValueError):
-        pass
-    return None
-
-
 def measured_peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         with open(p) as f:
             d = json.load(f)
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (HBM3, 3.35 TB/s)"
 
 
 class ClockSampler:
@@ -203,8 +190,7 @@ def host_pass_priorities(groups, bits, plc):
     """(encoder, decoder) stream priorities of the host-buffer pass; LYRA_BENCH_HOST_ENC_PRIORITY / ..._DEC_PRIORITY override.
     Equal by default (the synchronous calls of the 3.2 kbps workload lose 2-3 % with the encoder first, and four worker groups do
     well with equal priorities at every bit rate).  With only two worker groups the longer encoder chain of the higher bit rates
-    (30 / 46 serial RVQ stages behind kernels A and B) holds the pipeline back and the encoder goes one step up: measured on one
-    B200, 2 groups, 6.0 / 9.2 kbps: 5.60 / 5.53 M frames/s end to end against 5.06 / 4.80 M with equal priorities."""
+    (30 / 46 serial RVQ stages behind kernels A and B) holds the pipeline back and the encoder goes one step up."""
     enc = -1 if (groups <= 2 and bits > 64 and not plc) else 0
     enc = int(os.environ.get("LYRA_BENCH_HOST_ENC_PRIORITY", str(enc)))
     dec = int(os.environ.get("LYRA_BENCH_HOST_DEC_PRIORITY", "0"))
@@ -307,7 +293,8 @@ def emit(line):
         os.write(_JSON_FD, data)
 
 
-def measure(args, n, bits, plc, loss, hops, warm_hops, kernel_hops, e2e_hops, world, rank, local_rank, decoder_mode, want_clocks):
+def measure(args, n, bits, plc, loss, hops, warm_hops, kernel_hops, e2e_hops, world, rank, local_rank, decoder_mode, want_clocks,
+            dump_dir=None):
     """One configuration on this rank's GPU: device-resident throughput over `hops` hops, a serialised per-kernel pass, and the
     end-to-end pass through the host-buffer C ABI.  Returns a dict; multi-rank reductions (max over ranks) are done inside."""
     import ctypes as C
@@ -327,9 +314,8 @@ def measure(args, n, bits, plc, loss, hops, warm_hops, kernel_hops, e2e_hops, wo
     for c in ctxs:
         c.set_split(args.split)
     # Stream priorities (lyra_b200_set_priority, include/lyra_b200.h).  The device-resident pass queues many hops ahead through the
-    # asynchronous *_device calls: there the encoder direction runs one step above the decoder (measured +2.8 % over equal
-    # priorities, -3 % with the decoder first).  The host-buffer pass makes synchronous calls: equal priorities (measured: the
-    # encoder-first setting costs it 2-3 %), so the encoder contexts go back to 0 before it.  Both settings are in `config`.
+    # asynchronous *_device calls: there the encoder direction runs one step above the decoder.  The host-buffer pass makes
+    # synchronous calls: equal priorities, so the encoder contexts go back to 0 before it.  Both settings are in `config`.
     prio_x = int(os.environ.get("LYRA_BENCH_DEVICE_ENC_PRIORITY", "-1"))
     prio_y = int(os.environ.get("LYRA_BENCH_DEVICE_DEC_PRIORITY", "0"))
     sx, sy = torch.cuda.Stream(priority=prio_x), torch.cuda.Stream(priority=prio_y)
@@ -363,8 +349,7 @@ def measure(args, n, bits, plc, loss, hops, warm_hops, kernel_hops, e2e_hops, wo
             groups.append((e_, d_, gx, gy))
     group_ctxs = [c for grp in groups for c in grp[:2] if c is not None]
     # the host-buffer pass has its own number of worker groups (--e2e-groups): synchronous calls need more call chains in flight to
-    # cover their host turn-arounds and the serial RVQ stages than the asynchronous device pass does (measured at 6.0 / 9.2 kbps:
-    # 4 groups 5.8 / 5.5 M frames/s end to end, 2 groups 5.1-5.5 / 4.7 M; the device pass is best at 2)
+    # cover their host turn-arounds and the serial RVQ stages than the asynchronous device pass does
     ranks_sharing = 1 if os.environ.get("LYRA_BENCH_PINNED") else world
     Gh = host_pass_groups(args.e2e_groups, plc, ranks_sharing, host_cores(), n)
     # it runs 2 Gh waiting threads per rank: they sleep instead of spin when the box has fewer cores than that
@@ -447,6 +432,14 @@ def measure(args, n, bits, plc, loss, hops, warm_hops, kernel_hops, e2e_hops, wo
     torch.cuda.synchronize()
     elapsed_ms = e0.elapsed_time(e1)
     clocks = sampler.stop() if sampler else None
+    if dump_dir:
+        # the last timed hop's results as a caller of the device-resident API receives them (every group wrote its slice)
+        import numpy as np
+        last = (hops - 1) % NBUF
+        outs = {"pcm": d_out, "flags": d_flags} if plc else {"pcm": d_out, "packets": d_pks[last]}
+        os.makedirs(dump_dir, exist_ok=True)
+        for name, tn in outs.items():
+            np.save(os.path.join(dump_dir, name + ".npy"), tn.cpu().numpy().astype(np.float32))
     gpu_launches = sum(c.launch_count for c in group_ctxs) - launches0
     barrier()
     # per-kernel roofline pass on the full-size context pair: the same hops with the kernels serialised (one launch per kernel
@@ -587,21 +580,21 @@ def roofline_of(res, n, bits, plc, world, hops, decoder_mode, clocks):
     total_algo = (74368 + 640 + P + 1 + 2 * 5 * 160 * 4 + 2 * 640) if plc else (79744 + 640 + P) + (74368 + 640 + P)
     whole = total_algo * n * hops / (res["elapsed_ms"] / 1e3) / 1e9 if world == 1 else None
     roofline = {"bound": "hbm", "kernel": dom, "achieved": kern[dom]["achieved_gbs"], "peak": peak, "unit": "GB/s",
-                "frac": kern[dom]["achieved_gbs"] / peak, "traffic": ncu_traffic(dom, n), "peak_source": peak_src,
+                "frac": kern[dom]["achieved_gbs"] / peak, "peak_source": peak_src,
                 "kernel_share_of_step": kern[dom]["ms_per_launch"] / sum(v["ms_per_launch"] for v in kern.values()),
                 "whole_step": {"algo_bytes_per_frame": total_algo, "achieved_gbs": whole, "frac": whole / peak if whole else None},
                 "kernels": kern}
     if world == 1:
         # the CUDA-core roofline that binds the bit-exact layers (DESIGN.md section 5): ordered FFMA chains.  In the tensor decoder mode
         # only the encoder's fp32 layers and the decoder's bottleneck_2 stay on the FP32 pipe; the rest of the decoder's fp32 GEMMs run
-        # on the tensor cores (kernel C: mma.sync TF32, kernel D: tcgen05 UMMA)
+        # on the tensor cores (kernel C: mma.sync TF32, kernel D: wgmma)
         enc_macs, dec_macs, dec_cuda_macs = 1475840, 1236736, 24576          # SURVEY.md section 8d, fp32 MACs per stream-frame
         fp32_macs = (0 if plc else enc_macs) + (dec_macs if decoder_mode == "exact" else dec_cuda_macs)
-        sm_mhz = (clocks or {}).get("sm_mhz") or 1965.0
-        pipe_peak = 148 * 128 * 2 * sm_mhz * 1e6 / 1e12
+        sm_mhz = (clocks or {}).get("sm_mhz") or 1980.0
+        pipe_peak = 132 * 128 * 2 * sm_mhz * 1e6 / 1e12
         roofline["fp32_pipe"] = {"achieved": res["value"] * 2 * fp32_macs / 1e12, "peak": pipe_peak, "unit": "TFLOP/s",
                                  "frac": res["value"] * 2 * fp32_macs / 1e12 / pipe_peak, "fp32_macs_per_frame_on_cuda_cores": fp32_macs,
-                                 "peak_source": "148 SMs x 128 FP32 lanes x 2 x SM clock sampled during the run"}
+                                 "peak_source": "132 SMs x 128 FP32 lanes x 2 x SM clock sampled during the run (H100 SXM)"}
     return roofline
 
 
@@ -636,8 +629,11 @@ def main():
                     help="synthetic input: uniform noise at 0.25 full scale (default) or the tiled reference speech clips")
     ap.add_argument("--host-wait", default="auto", choices=["auto", "spin", "sleep"],
                     help="how the worker threads of the host-buffer pass wait for the GPU (auto: sleep only when threads outnumber cores)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write what the last timed hop returned to its caller (decoded PCM, packets; "
+                         "decode_plc: PCM and comfort-noise flags) as DIR/<name>.npy in float32")
     ap.add_argument("--decoder-mode", default="tensor", choices=["exact", "tensor"],
-                    help="tensor (default): the decoder's fp32 GEMMs on the tensor cores (kernel D: tcgen05 UMMA), decoded PCM within "
+                    help="tensor (default): the decoder's fp32 GEMMs on the tensor cores (kernel D: wgmma), decoded PCM within "
                          "4 int16 LSB of the oracle, packets bit-exact; exact: decoded PCM bit-identical to the oracle")
     args = ap.parse_args()
     if args.bits is None:
@@ -655,7 +651,7 @@ def main():
     import torch.distributed as dist
 
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py: no CUDA device (the B200 path has no CPU fallback; use --impl reference for the CPU arm)")
+        raise SystemExit("bench.py: no CUDA device (the CUDA path has no CPU fallback; use --impl reference for the CPU arm)")
     torch.cuda.set_device(local_rank)
     pinned = pin_rank_cores(local_rank, int(os.environ.get("LOCAL_WORLD_SIZE", str(world))))
     if world > 1:
@@ -664,8 +660,11 @@ def main():
     n, bits = args.streams, args.bits
     plc = args.workload == "decode_plc"
     hops = args.steps * HOPS_PER_STEP
+    dump_dir = None
+    if args.dump_outputs:
+        dump_dir = args.dump_outputs if world == 1 else os.path.join(args.dump_outputs, "rank%d" % rank)
     res = measure(args, n, bits, plc, args.loss, hops, max(3, args.warmup) * HOPS_PER_STEP, min(hops, 40), hops, world, rank, local_rank,
-                  args.decoder_mode, want_clocks=True)
+                  args.decoder_mode, want_clocks=True, dump_dir=dump_dir)
     value, e2e_value, clocks, P, G = res["value"], res["e2e_value"], res["clocks"], res["P"], res["G"]
 
     other = None
@@ -719,9 +718,9 @@ def main():
                        "host_threads_wait": "sleep (blocking-sync event)" if res["oversubscribed"] else "spin",
                        "host_cores_per_rank": pinned if pinned else host_cores(),
                        "real_time_factor": value / (50.0 * n * world),
-                       "l2": ("no flush needed: per-hop state working set %d x %.0f KB = %.0f MB exceeds the 126 MB L2; PCM inputs rotate over 8 buffers"
-                              if state_mb > 126 else
-                              "NOT flushed: the state working set %d x %.0f KB = %.0f MB fits in the 126 MB L2 at this stream count (as it would "
+                       "l2": ("no flush needed: per-hop state working set %d x %.0f KB = %.0f MB exceeds the 50 MB L2; PCM inputs rotate over 8 buffers"
+                              if state_mb > 50 else
+                              "NOT flushed: the state working set %d x %.0f KB = %.0f MB fits in the 50 MB L2 at this stream count (as it would "
                               "in steady-state serving); PCM inputs rotate over 8 buffers; the headline configuration (4096 streams) exceeds L2")
                              % (n, EncDecStateBytes() / 1024.0, state_mb),
                        "parallelism": "streams sharded by rank, no data-path collective",

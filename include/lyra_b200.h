@@ -1,5 +1,5 @@
 /*
- * lyra_b200 — C ABI of the B200-native Lyra v1.3.2 hot path.
+ * lyra_b200 — C ABI of the H100-native Lyra v1.3.2 hot path.
  *
  * This is the seam that replaces `TfLiteModelWrapper` (reference: lyra/tflite_model_wrapper.h:32-67)
  * underneath the three plugin classes bound in lyra/lyra_components.cc:42-55.  Plain pointers and
@@ -201,10 +201,10 @@ int lyra_b200_decoder_mode(const lyra_b200_ctx* ctx);
  * CUDA event — for servers that run more waiting worker threads than they have cores. */
 int lyra_b200_set_blocking_sync(lyra_b200_ctx* ctx, int enable);
 /* CUDA priority of the context's own stream and of its sub-batch streams (0 = default, negative = higher; the device clamps).
- * A process that runs an encoder-only and a decoder-only context side by side through the asynchronous *_device calls gains
- * about 3 % of throughput with the encoder one step above the decoder (the uplink chain is the longer one; its blocks go
- * first, the decoder's latency-bound blocks fill what is left); with the synchronous host-buffer calls equal priorities are
- * the better choice (measured, DESIGN.md section 6).  Waits for the context's work, re-creates the streams, drops captured
+ * A process that runs an encoder-only and a decoder-only context side by side through the asynchronous *_device calls can
+ * run the encoder one step above the decoder (the uplink chain is the longer one; its blocks go first, the decoder's
+ * latency-bound blocks fill what is left); with the synchronous host-buffer calls equal priorities are the better choice
+ * (DESIGN.md section 6).  Waits for the context's work, re-creates the streams, drops captured
  * graphs.  A caller stream installed with lyra_b200_set_stream keeps its own priority.  Default 0, or the environment
  * variables LYRA_B200_ENC_PRIORITY / LYRA_B200_DEC_PRIORITY at creation. */
 int lyra_b200_set_priority(lyra_b200_ctx* ctx, int priority);

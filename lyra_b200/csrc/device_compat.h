@@ -1,4 +1,4 @@
-// Build-mode shim.  The product is compiled by nvcc for sm_100a.  The same kernel sources are also
+// Build-mode shim.  The product is compiled by nvcc for sm_90a.  The same kernel sources are also
 // compiled by g++ with -DLYRA_EMU against tests/cuda_emu (a test-only CPU block simulator) so the
 // CPU test tier can check kernel logic against the oracle without a GPU.  Nothing in the shipped
 // library depends on the emulator.
@@ -73,11 +73,6 @@ static inline void lyra_bulk_g2s(void* smem_dst, const void* gmem_src, unsigned 
 static inline void lyra_mbar_wait(LyraMbar* b, unsigned parity) {
   while (lyra_mbar_emu(b)->phase == parity) cuda_emu::yield();
 }
-// several bulk copies completing ONE barrier phase: begin(total bytes), copy ..., end (the emulated copies are synchronous, so
-// the single arrival is counted by end; on the GPU begin arms the barrier and end is a no-op)
-static inline void lyra_bulk_multi_begin(LyraMbar*, unsigned) {}
-static inline void lyra_bulk_multi_copy(void* smem_dst, const void* gmem_src, unsigned bytes, LyraMbar*) { std::memcpy(smem_dst, gmem_src, bytes); }
-static inline void lyra_bulk_multi_end(LyraMbar* b) { lyra_mbar_arrive(b); }
 // one function-local shared object per kernel (the emulator backs them all with the same per-block scratch area)
 #define LYRA_STATIC_SMEM(type, name, count) \
   static_assert(sizeof(type) * (count) <= 448, "emulated static shared memory: 448 bytes for objects + 64 for named barriers"); \
@@ -106,14 +101,6 @@ __device__ __forceinline__ void lyra_bulk_g2s(void* smem_dst, const void* gmem_s
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];\n"
                ::"r"(lyra_smem_u32(smem_dst)), "l"(gmem_src), "r"(bytes), "r"(bar) : "memory");
 }
-__device__ __forceinline__ void lyra_bulk_multi_begin(LyraMbar* b, unsigned total_bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;\n" ::"r"(lyra_smem_u32(b)), "r"(total_bytes) : "memory");
-}
-__device__ __forceinline__ void lyra_bulk_multi_copy(void* smem_dst, const void* gmem_src, unsigned bytes, LyraMbar* b) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];\n"
-               ::"r"(lyra_smem_u32(smem_dst)), "l"(gmem_src), "r"(bytes), "r"(lyra_smem_u32(b)) : "memory");
-}
-__device__ __forceinline__ void lyra_bulk_multi_end(LyraMbar*) {}
 __device__ __forceinline__ void lyra_mbar_wait(LyraMbar* b, unsigned parity) {
   const unsigned bar = lyra_smem_u32(b);
   asm volatile("{\n"
@@ -199,214 +186,87 @@ __device__ __forceinline__ void lyra_mma_tf32_16x8x8(float (&c)[4], const uint32
 }
 #endif
 
-// ---- 5th-generation tensor cores (tcgen05 / UMMA) with accumulators in tensor memory (TMEM).
-//      Not used by the shipped kernels yet (DESIGN.md section 9): these wrappers carry the instruction sequences that
-//      tools/tcgen05_probe.cu verified on a B200, plus an emulator model so the CPU test tier can run UMMA kernels.
-//      Shared-memory matrix descriptor (no swizzle, K-major): element (row, k) of an operand lives at
-//        start + (k / 4) * LBO + (row / 8) * SBO + (row % 8) * 16 + (k % 4) * 4   bytes
+// ---- warpgroup MMA (wgmma, sm_90a): D[64 x N] (+)= A[64 x 8] * B[N x 8]^T in TF32 with fp32 accumulators in the registers of
+//      the four warps of a warpgroup (128 consecutive threads, the first a multiple of 128).  The MMA reads the top 19 bits of
+//      every operand.  Shared-memory operands are K-major without swizzle, addressed by a matrix descriptor:
+//        element (row, k) at start + (k / 4) * LBO + (row / 8) * SBO + (row % 8) * 16 + (k % 4) * 4   bytes
 //      i.e. 8-row x 16-byte core matrices, LBO = byte distance of the two 4-element k-halves of one MMA (K = 8),
-//      SBO = byte distance of consecutive 8-row groups.  kind::tf32 reads the top 19 bits of every operand.
-//      TMEM address = (lane << 16) | column; an M = 128 accumulator puts row r in lane r, column n in column n.
-__host__ __device__ inline uint32_t lyra_umma_idesc_tf32(int M, int N) {
-  // D = f32 (bits 4-5 = 1), A = B = tf32 (bits 7-9, 10-12 = 2), both K-major, N >> 3 at bit 17, M >> 4 at bit 24
-  return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
+//      SBO = byte distance of consecutive 8-row groups.
+//      Register fragments (warp q of the warpgroup, g = lane / 4, t = lane % 4):
+//        A:  a0 (16q + g, t)   a1 (16q + g + 8, t)   a2 (16q + g, t + 4)   a3 (16q + g + 8, t + 4)
+//        D:  d[4j] (16q + g, 8j + 2t)   d[4j + 1] (16q + g, 8j + 2t + 1)   d[4j + 2] (16q + g + 8, 8j + 2t)   d[4j + 3] (16q + g + 8, 8j + 2t + 1)
+//      Issue order: lyra_wgmma_fence() before the first MMA that touches registers written since, the MMAs, lyra_wgmma_commit(),
+//      and lyra_wgmma_wait<0>() before the accumulators are read or a shared-memory operand is overwritten.
 #if defined(LYRA_EMU)
 static inline uint32_t lyra_emu_smem_addr(const void* p) { return (uint32_t)(reinterpret_cast<const char*>(p) - cuda_emu::g_blk->smem); }
-static inline uint64_t lyra_umma_desc(const void* smem, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+static inline uint64_t lyra_wgmma_desc(const void* smem, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   return (uint64_t)((lyra_emu_smem_addr(smem) >> 4) & 0x3FFF) | (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16 |
-         (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32 | (uint64_t)1 << 46;
+         (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
 }
-static inline float* lyra_emu_tmem(uint32_t taddr, int lane_add, int col_add) {
-  cuda_emu::BlockState* b = cuda_emu::g_blk;
-  if (b->tmem.empty()) b->tmem.assign(128 * 512, 0.0f);
-  const unsigned lane = (taddr >> 16) + (unsigned)lane_add, col = (taddr & 0xffffu) + (unsigned)col_add;
-  if (lane >= 128 || col >= 512) { std::fprintf(stderr, "cuda_emu: TMEM access out of range (lane %u, column %u)\n", lane, col); std::abort(); }
-  return &b->tmem[(size_t)lane * 512 + col];
-}
-// warp-collective in hardware; here every lane of the calling warp runs it and lane 0 does the work
-static inline void lyra_tmem_alloc(uint32_t* smem_slot, int ncols) {
-  if ((threadIdx.x & 31) == 0) {
-    cuda_emu::BlockState* b = cuda_emu::g_blk;
-    if (ncols < 32 || (ncols & (ncols - 1)) || b->tmem_used + (unsigned)ncols > 512) { std::fprintf(stderr, "cuda_emu: bad TMEM allocation\n"); std::abort(); }
-    *smem_slot = b->tmem_used;
-    b->tmem_used += (unsigned)ncols;
-  }
-  __syncwarp();
-}
-static inline void lyra_tmem_dealloc(uint32_t, int) { __syncwarp(); }
-static inline void lyra_tc_fence_before_sync() {}
-static inline void lyra_tc_fence_after_sync() {}
-// D[M x N] (+)= A[M x 8] * B[N x 8]^T, one thread issues it; the emulator executes it on the spot
-static inline void lyra_umma_tf32(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, bool accumulate) {
-  const int N = (int)((idesc >> 17) & 0x3f) << 3, M = (int)((idesc >> 24) & 0x1f) << 4;
-  const char* base = cuda_emu::g_blk->smem;
-  auto elem = [&](uint64_t d, int row, int k) {
-    const uint32_t start = (uint32_t)(d & 0x3FFF) << 4, lbo = (uint32_t)((d >> 16) & 0x3FFF) << 4, sbo = (uint32_t)((d >> 32) & 0x3FFF) << 4;
-    uint32_t bits;
-    std::memcpy(&bits, base + start + (uint32_t)(k / 4) * lbo + (uint32_t)(row / 8) * sbo + (uint32_t)(row % 8) * 16 + (uint32_t)(k % 4) * 4, 4);
-    return (double)lyra_emu_tf32(bits);
-  };
-  for (int m = 0; m < M; ++m)
-    for (int n = 0; n < N; ++n) {
-      double acc = accumulate ? (double)*lyra_emu_tmem(tmem_d, m, n) : 0.0;
-      for (int k = 0; k < 8; ++k) acc += elem(desc_a, m, k) * elem(desc_b, n, k);
-      *lyra_emu_tmem(tmem_d, m, n) = (float)acc;
-    }
-}
-// all MMAs issued so far by this thread are complete when the barrier's phase completes
-static inline void lyra_umma_commit(LyraMbar* b) { lyra_mbar_arrive(b); }
-// 32x32b shape: lane i of the warp reads TMEM lane (address lane) + i, 8 consecutive columns
-static inline void lyra_tmem_ld8(uint32_t taddr, float (&v)[8]) {
-  const int lane = (int)(threadIdx.x & 31), warp = (int)(threadIdx.x >> 5);
-  if ((taddr >> 16) != (uint32_t)(32 * (warp % 4))) {      // hardware rule: warp w of a warpgroup reaches TMEM lanes 32 (w % 4) .. + 31 only
-    std::fprintf(stderr, "cuda_emu: warp %d may not read TMEM lanes starting at %u\n", warp, taddr >> 16);
-    std::abort();
-  }
-  for (int j = 0; j < 8; ++j) v[j] = *lyra_emu_tmem(taddr, lane, j);
-}
-
-// ---- additions for the product's UMMA kernels: A operand in TMEM, kind::i8, tcgen05.st, wide tcgen05.ld ----
-static inline uint32_t* lyra_emu_tmem_u32(uint32_t taddr, int lane_add, int col_add) { return reinterpret_cast<uint32_t*>(lyra_emu_tmem(taddr, lane_add, col_add)); }
-static inline void lyra_emu_check_lane_window(uint32_t taddr) {
-  const int warp = (int)(threadIdx.x >> 5);
-  if ((taddr >> 16) != (uint32_t)(32 * (warp % 4))) {
-    std::fprintf(stderr, "cuda_emu: warp %d may not access TMEM lanes starting at %u\n", warp, taddr >> 16);
-    std::abort();
-  }
-}
-// D[M x N] (+)= A[M x 8] * B[N x 8]^T with A in TMEM: row r of A is TMEM lane r, element k is column (address column) + k
-static inline void lyra_umma_tf32_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc, bool accumulate) {
-  const int N = (int)((idesc >> 17) & 0x3f) << 3, M = (int)((idesc >> 24) & 0x1f) << 4;
-  const char* base = cuda_emu::g_blk->smem;
-  auto belem = [&](int row, int k) {
-    const uint32_t start = (uint32_t)(desc_b & 0x3FFF) << 4, lbo = (uint32_t)((desc_b >> 16) & 0x3FFF) << 4, sbo = (uint32_t)((desc_b >> 32) & 0x3FFF) << 4;
-    uint32_t bits;
-    std::memcpy(&bits, base + start + (uint32_t)(k / 4) * lbo + (uint32_t)(row / 8) * sbo + (uint32_t)(row % 8) * 16 + (uint32_t)(k % 4) * 4, 4);
-    return (double)lyra_emu_tf32(bits);
-  };
-  for (int m = 0; m < M; ++m)
-    for (int n = 0; n < N; ++n) {
-      double acc = accumulate ? (double)*lyra_emu_tmem(tmem_d, m, n) : 0.0;
-      for (int k = 0; k < 8; ++k) acc += (double)lyra_emu_tf32(*lyra_emu_tmem_u32(tmem_a, m, k)) * belem(n, k);
-      *lyra_emu_tmem(tmem_d, m, n) = (float)acc;
-    }
-}
-// kind::i8: D (s32) [M x N] (+)= A (s8) [M x 32] * B (s8) [N x 32]^T; K-major no-swizzle operands are 8-row x 16-byte core
-// matrices: element (row, k) at start + (k / 16) * LBO + (row / 8) * SBO + (row % 8) * 16 + k % 16 bytes
-__host__ __device__ inline uint32_t lyra_umma_idesc_i8(int M, int N) {
-  return (2u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);   // D = s32, A = B = s8
-}
-static inline int lyra_emu_i8_elem(uint64_t d, int row, int k) {
-  const char* base = cuda_emu::g_blk->smem;
+static inline double lyra_emu_desc_elem(uint64_t d, int row, int k) {
   const uint32_t start = (uint32_t)(d & 0x3FFF) << 4, lbo = (uint32_t)((d >> 16) & 0x3FFF) << 4, sbo = (uint32_t)((d >> 32) & 0x3FFF) << 4;
-  return (int)*reinterpret_cast<const int8_t*>(base + start + (uint32_t)(k / 16) * lbo + (uint32_t)(row / 8) * sbo + (uint32_t)(row % 8) * 16 + (uint32_t)(k % 16));
+  uint32_t bits;
+  std::memcpy(&bits, cuda_emu::g_blk->smem + start + (uint32_t)(k / 4) * lbo + (uint32_t)(row / 8) * sbo + (uint32_t)(row % 8) * 16 + (uint32_t)(k % 4) * 4, 4);
+  return (double)lyra_emu_tf32(bits);
 }
-static inline void lyra_umma_i8(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, bool accumulate) {
-  const int N = (int)((idesc >> 17) & 0x3f) << 3, M = (int)((idesc >> 24) & 0x1f) << 4;
-  for (int m = 0; m < M; ++m)
-    for (int n = 0; n < N; ++n) {
-      int32_t* d = reinterpret_cast<int32_t*>(lyra_emu_tmem(tmem_d, m, n));
-      int acc = accumulate ? *d : 0;
-      for (int k = 0; k < 32; ++k) acc += lyra_emu_i8_elem(desc_a, m, k) * lyra_emu_i8_elem(desc_b, n, k);
-      *d = acc;
-    }
+// the emulated MMA completes on the spot: fence, commit and wait have nothing to order
+static inline void lyra_wgmma_fence() {}
+static inline void lyra_wgmma_commit() {}
+template <int N>
+static inline void lyra_wgmma_wait() {}
+// every thread computes its own accumulator fragment from the shared-memory operands
+static inline void lyra_wgmma_m64n32_tf32_ss(float (&d)[16], uint64_t desc_a, uint64_t desc_b, bool accumulate) {
+  const int lane = (int)(threadIdx.x & 31), q = (int)((threadIdx.x >> 5) & 3), g = lane >> 2, t = lane & 3;
+  for (int i = 0; i < 16; ++i) {
+    const int row = 16 * q + g + 8 * ((i >> 1) & 1), col = 8 * (i >> 2) + 2 * t + (i & 1);
+    double acc = accumulate ? (double)d[i] : 0.0;
+    for (int k = 0; k < 8; ++k) acc += lyra_emu_desc_elem(desc_a, row, k) * lyra_emu_desc_elem(desc_b, col, k);
+    d[i] = (float)acc;
+  }
 }
-// A (s8) in TMEM: row r is lane r, 4 consecutive k per 32-bit column (little endian), 8 columns per MMA
-static inline void lyra_umma_i8_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc, bool accumulate) {
-  const int N = (int)((idesc >> 17) & 0x3f) << 3, M = (int)((idesc >> 24) & 0x1f) << 4;
-  for (int m = 0; m < M; ++m)
-    for (int n = 0; n < N; ++n) {
-      int32_t* d = reinterpret_cast<int32_t*>(lyra_emu_tmem(tmem_d, m, n));
-      int acc = accumulate ? *d : 0;
-      for (int k = 0; k < 32; ++k) acc += (int)(int8_t)((*lyra_emu_tmem_u32(tmem_a, m, k / 4) >> (8 * (k % 4))) & 0xff) * lyra_emu_i8_elem(desc_b, n, k);
-      *d = acc;
-    }
+// A from registers: a warp's 16 rows of A are its own fragments, so the warp's lanes exchange theirs
+static inline void lyra_wgmma_m64n64_tf32_rs(float (&d)[32], const uint32_t (&a)[4], uint64_t desc_b, bool accumulate) {
+  const uint32_t (*all)[8] = cuda_emu::warp_gather(a, 4);
+  const int lane = (int)(threadIdx.x & 31), g = lane >> 2, t = lane & 3;
+  auto A = [&](int row, int k) { return (double)lyra_emu_tf32(all[(row & 7) * 4 + (k & 3)][(row >> 3) + 2 * (k >> 2)]); };
+  float out[32];
+  for (int i = 0; i < 32; ++i) {
+    const int row = g + 8 * ((i >> 1) & 1), col = 8 * (i >> 2) + 2 * t + (i & 1);
+    double acc = accumulate ? (double)d[i] : 0.0;
+    for (int k = 0; k < 8; ++k) acc += A(row, k) * lyra_emu_desc_elem(desc_b, col, k);
+    out[i] = (float)acc;
+  }
+  cuda_emu::warp_barrier();             // keep the table alive until every lane has read it
+  for (int i = 0; i < 32; ++i) d[i] = out[i];
 }
-template <int NC>
-static inline void lyra_tmem_ld(uint32_t taddr, uint32_t (&v)[NC]) {
-  lyra_emu_check_lane_window(taddr);
-  const int lane = (int)(threadIdx.x & 31);
-  for (int j = 0; j < NC; ++j) v[j] = *lyra_emu_tmem_u32(taddr, lane, j);
-}
-template <int NC>
-static inline void lyra_tmem_st(uint32_t taddr, const uint32_t (&v)[NC]) {
-  lyra_emu_check_lane_window(taddr);
-  const int lane = (int)(threadIdx.x & 31);
-  for (int j = 0; j < NC; ++j) *lyra_emu_tmem_u32(taddr, lane, j) = v[j];
-}
-static inline void lyra_tmem_wait_ld() {}
-static inline void lyra_tmem_wait_st() {}
 #elif defined(__CUDACC__)
-__device__ __forceinline__ uint64_t lyra_umma_desc(const void* smem, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+__device__ __forceinline__ uint64_t lyra_wgmma_desc(const void* smem, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   return (uint64_t)((lyra_smem_u32(smem) >> 4) & 0x3FFF) | (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16 |
-         (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32 | (uint64_t)1 << 46;     // descriptor version 1, no swizzle
+         (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;                 // layout type 0: no swizzle
 }
-// one whole warp; ncols a power of two >= 32; the TMEM base address is written to *smem_slot (shared memory)
-__device__ __forceinline__ void lyra_tmem_alloc(uint32_t* smem_slot, int ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;\n" ::"r"(lyra_smem_u32(smem_slot)), "r"(ncols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;\n" ::: "memory");
+__device__ __forceinline__ void lyra_wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;\n" ::: "memory"); }
+__device__ __forceinline__ void lyra_wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;\n" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void lyra_wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;\n" ::"n"(N) : "memory"); }
+__device__ __forceinline__ void lyra_wgmma_m64n32_tf32_ss(float (&d)[16], uint64_t desc_a, uint64_t desc_b, bool accumulate) {
+  asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %18, 0;\n"
+               "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 "
+               "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1;\n}\n"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+                 "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+               : "l"(desc_a), "l"(desc_b), "r"(accumulate ? 1u : 0u));
 }
-__device__ __forceinline__ void lyra_tmem_dealloc(uint32_t taddr, int ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;\n" ::"r"(taddr), "r"(ncols) : "memory");
+__device__ __forceinline__ void lyra_wgmma_m64n64_tf32_rs(float (&d)[32], const uint32_t (&a)[4], uint64_t desc_b, bool accumulate) {
+  asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %37, 0;\n"
+               "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
+               "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, "
+               "{%32,%33,%34,%35}, %36, p, 1, 1;\n}\n"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+                 "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+                 "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+                 "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"(accumulate ? 1u : 0u));
 }
-__device__ __forceinline__ void lyra_tc_fence_before_sync() { asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory"); }
-__device__ __forceinline__ void lyra_tc_fence_after_sync() { asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory"); }
-__device__ __forceinline__ void lyra_umma_tf32(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, bool accumulate) {
-  asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\ntcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n}\n"
-               ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate ? 1u : 0u) : "memory");
-}
-__device__ __forceinline__ void lyra_umma_commit(LyraMbar* b) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n" ::"r"(lyra_smem_u32(b)) : "memory");
-}
-__device__ __forceinline__ void lyra_tmem_ld8(uint32_t taddr, float (&v)[8]) {
-  uint32_t r[8];
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];\n"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]) : "r"(taddr) : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;\n" ::: "memory");
-#pragma unroll
-  for (int j = 0; j < 8; ++j) v[j] = __uint_as_float(r[j]);
-}
-
-__host__ __device__ inline uint32_t lyra_umma_idesc_i8(int M, int N) {
-  return (2u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);   // D = s32, A = B = s8
-}
-__device__ __forceinline__ void lyra_umma_tf32_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc, bool accumulate) {
-  asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\ntcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, p;\n}\n"
-               ::"r"(tmem_d), "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate ? 1u : 0u) : "memory");
-}
-__device__ __forceinline__ void lyra_umma_i8(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, bool accumulate) {
-  asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\ntcgen05.mma.cta_group::1.kind::i8 [%0], %1, %2, %3, p;\n}\n"
-               ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate ? 1u : 0u) : "memory");
-}
-__device__ __forceinline__ void lyra_umma_i8_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc, bool accumulate) {
-  asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\ntcgen05.mma.cta_group::1.kind::i8 [%0], [%1], %2, %3, p;\n}\n"
-               ::"r"(tmem_d), "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate ? 1u : 0u) : "memory");
-}
-// 32x32b shape, NC consecutive columns: lane i of the warp accesses TMEM lane (address lane) + i.  The loaded registers are valid
-// after lyra_tmem_wait_ld(); stored data is visible to later MMAs after lyra_tmem_wait_st() (+ the usual fences).
-template <int NC> __device__ __forceinline__ void lyra_tmem_ld(uint32_t taddr, uint32_t (&v)[NC]);
-template <> __device__ __forceinline__ void lyra_tmem_ld<8>(uint32_t taddr, uint32_t (&r)[8]) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];\n"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]) : "r"(taddr) : "memory");
-}
-template <> __device__ __forceinline__ void lyra_tmem_ld<16>(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];\n"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-                 "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]) : "r"(taddr) : "memory");
-}
-template <int NC> __device__ __forceinline__ void lyra_tmem_st(uint32_t taddr, const uint32_t (&v)[NC]);
-template <> __device__ __forceinline__ void lyra_tmem_st<8>(uint32_t taddr, const uint32_t (&r)[8]) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};\n"
-               ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]) : "memory");
-}
-template <> __device__ __forceinline__ void lyra_tmem_st<16>(uint32_t taddr, const uint32_t (&r)[16]) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16};\n"
-               ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]),
-                 "r"(r[8]), "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]) : "memory");
-}
-__device__ __forceinline__ void lyra_tmem_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;\n" ::: "memory"); }
-__device__ __forceinline__ void lyra_tmem_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;\n" ::: "memory"); }
 #endif
 
 // ---- bulk asynchronous store shared -> global (TMA, cp.async.bulk.global.shared::cta) and named barriers for warp subsets.
@@ -439,33 +299,3 @@ __device__ __forceinline__ void lyra_bulk_wait_read() { asm volatile("cp.async.b
 __device__ __forceinline__ void lyra_bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;\n" ::: "memory"); }
 __device__ __forceinline__ void lyra_named_bar_sync(int id, int nthreads) { asm volatile("bar.sync %0, %1;\n" ::"r"(id), "r"(nthreads) : "memory"); }
 #endif
-
-// ---- thread-block clusters: a pair of CTAs shares one weight stream (each CTA's producer loads half of every chunk and TMA
-//      multicasts it into both CTAs' shared memory; a stage is recycled when BOTH CTAs' MMAs have released it).  The emulator
-//      runs one block at a time: clusters do not exist there and kernels take their single-CTA path.
-#if defined(LYRA_EMU)
-static inline unsigned lyra_cluster_ctarank() { return 0; }
-static inline unsigned lyra_cluster_nctarank() { return 1; }
-static inline void lyra_cluster_sync() {}
-static inline void lyra_bulk_g2s_mc(void* smem_dst, const void* gmem_src, unsigned bytes, LyraMbar*, unsigned) { std::memcpy(smem_dst, gmem_src, bytes); }
-static inline void lyra_umma_commit_mc(LyraMbar* b, unsigned) { lyra_mbar_arrive(b); }
-#elif defined(__CUDACC__)
-__device__ __forceinline__ unsigned lyra_cluster_ctarank() { unsigned r; asm volatile("mov.u32 %0, %%cluster_ctarank;\n" : "=r"(r)); return r; }
-__device__ __forceinline__ unsigned lyra_cluster_nctarank() { unsigned r; asm volatile("mov.u32 %0, %%cluster_nctarank;\n" : "=r"(r)); return r; }
-__device__ __forceinline__ void lyra_cluster_sync() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;\n" ::: "memory");
-}
-// bulk copy global -> the same shared-memory offset of every CTA in `cta_mask`; completes `bytes` of transaction count on the
-// mbarrier at the same offset in each of them (the barriers are armed by their own CTAs, see lyra_bulk_multi_begin)
-__device__ __forceinline__ void lyra_bulk_g2s_mc(void* smem_dst, const void* gmem_src, unsigned bytes, LyraMbar* b, unsigned cta_mask) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1], %2, [%3], %4;\n"
-               ::"r"(lyra_smem_u32(smem_dst)), "l"(gmem_src), "r"(bytes), "r"(lyra_smem_u32(b)), "h"((unsigned short)cta_mask) : "memory");
-}
-// tcgen05.commit that arrives on the mbarrier at this offset in every CTA of `cta_mask`
-__device__ __forceinline__ void lyra_umma_commit_mc(LyraMbar* b, unsigned cta_mask) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;\n"
-               ::"r"(lyra_smem_u32(b)), "h"((unsigned short)cta_mask) : "memory");
-}
-#endif
-

@@ -1,5 +1,5 @@
 // Context + launch logic + the C ABI of include/lyra_b200.h.
-// Compiled by nvcc for sm_100a (product) and, for the CPU test tier only, by g++ with -DLYRA_EMU.
+// Compiled by nvcc for sm_90a (product) and, for the CPU test tier only, by g++ with -DLYRA_EMU.
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
@@ -11,7 +11,7 @@
 #include "aux_kernels.cuh"
 #include "model_spec.h"
 #include "net_kernels.cuh"
-#include "net_kernels_umma.cuh"
+#include "net_kernels_wgmma.cuh"
 #include "plc_kernels.cuh"
 
 using namespace lyra_b200;
@@ -77,9 +77,6 @@ struct lyra_b200_ctx {
   int16_t* d_cng_pcm = nullptr;
   float* d_cng_feat = nullptr;
   const uint8_t* cur_skip = nullptr;         // skip mask of the call in flight (TileIo::skip)
-  bool du_cluster = false;                   // DecoderKernelDU in clusters of two CTAs sharing the weight stream by TMA multicast
-                                             // (LYRA_B200_DU_CLUSTER=1).  Measured on B200: no gain (0.203 vs 0.197 ms) - the stream is bound by
-                                             // the delivery into the SMs, not by L2 reads - so it is off by default; kept for parts where it pays
   // sample-rate converters: [direction 0 = to 16 kHz (encoder side), 1 = from 16 kHz (decoder side)][max_streams] state
   int16_t* d_rs_delay[2] = {nullptr, nullptr};   // [max_streams][34]
   int* d_rs_pos[2] = {nullptr, nullptr};         // [max_streams][2] {position, rate}
@@ -304,43 +301,24 @@ int LaunchDecoderNetsT(lyra_b200_ctx* ctx, const Part& p, const float* d_feature
   CU(cudaGetLastError());
   return LYRA_B200_OK;
 }
-// Tensor mode at 8-stream tiles (the default tile): kernel C with its fp32 residual units on mma.sync TF32, kernel D on the
-// 5th-generation tensor cores (tcgen05.mma, accumulators and A operands in tensor memory; net_kernels_umma.cuh).
-int LaunchDecoderNetsUmma(lyra_b200_ctx* ctx, const Part& p, const float* d_features, int16_t* d_pcm) {
+// Tensor mode at 8-stream tiles (the default tile): kernel C with its fp32 residual units on mma.sync TF32, kernel D on warpgroup
+// MMAs (wgmma, A operands and accumulators in registers; net_kernels_wgmma.cuh).
+int LaunchDecoderNetsWgmma(lyra_b200_ctx* ctx, const Part& p, const float* d_features, int16_t* d_pcm) {
   const TileIo io{ctx->d_tile_list + p.tile0, ctx->d_slot_of, ctx->cur_skip};
   using LC = DecC<8, true>;
   { ProfScope ps(ctx, 4, p.st);
   LYRA_LAUNCH((DecoderKernelC<8, true>), dim3((unsigned)p.ntiles), dim3(LC::NT), (size_t)LC::kSmemBytes, p.st,
               ctx->d_blob, ctx->spec.dec, io, d_features, reinterpret_cast<float*>(ctx->d_state[2]), ctx->d_n18[2], ctx->d_mid_dec); }
   { ProfScope ps(ctx, 5, p.st);
-#ifdef LYRA_EMU
-  LYRA_LAUNCH(DecoderKernelDU, dim3((unsigned)p.ntiles), dim3(DecDU::NT), (size_t)DecDU::kSmemBytes, p.st,
-              ctx->d_blob, ctx->spec.dec, io, ctx->d_mid_dec, reinterpret_cast<float*>(ctx->d_state[3]), ctx->d_n18[3], d_pcm, p.ntiles);
-#else
-  // clusters of two CTAs share the weight stream by TMA multicast (net_kernels_umma.cuh); an odd tile count gets one padding block
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3((unsigned)((p.ntiles + 1) / 2 * 2));
-  cfg.blockDim = dim3(DecDU::NT);
-  cfg.dynamicSmemBytes = (size_t)DecDU::kSmemBytes;
-  cfg.stream = p.st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = ctx->du_cluster ? 2 : 1;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  CU(cudaLaunchKernelEx(&cfg, DecoderKernelDU, (const uint8_t*)ctx->d_blob, ctx->spec.dec, io, (const float*)ctx->d_mid_dec,
-                        reinterpret_cast<float*>(ctx->d_state[3]), ctx->d_n18[3], d_pcm, p.ntiles));
-#endif
-  }
+  LYRA_LAUNCH(DecoderKernelDW, dim3((unsigned)p.ntiles), dim3(DecDW::NT), (size_t)DecDW::kSmemBytes, p.st,
+              ctx->d_blob, ctx->spec.dec, io, ctx->d_mid_dec, reinterpret_cast<float*>(ctx->d_state[3]), ctx->d_n18[3], d_pcm); }
   ctx->launches += 2;
   CU(cudaGetLastError());
   return LYRA_B200_OK;
 }
 int LaunchDecoderNets(lyra_b200_ctx* ctx, const Part& p, const float* d_features, int16_t* d_pcm) {
   const bool tc = ctx->decoder_mode == LYRA_B200_DECODER_TENSOR;
-  if (tc && ctx->S == 8) return LaunchDecoderNetsUmma(ctx, p, d_features, d_pcm);
+  if (tc && ctx->S == 8) return LaunchDecoderNetsWgmma(ctx, p, d_features, d_pcm);
   if (ctx->S == 16) return tc ? LaunchDecoderNetsT<16, true>(ctx, p, d_features, d_pcm) : LaunchDecoderNetsT<16, false>(ctx, p, d_features, d_pcm);
   return tc ? LaunchDecoderNetsT<8, true>(ctx, p, d_features, d_pcm) : LaunchDecoderNetsT<8, false>(ctx, p, d_features, d_pcm);
 }
@@ -348,7 +326,7 @@ int LaunchDecoderNets(lyra_b200_ctx* ctx, const Part& p, const float* d_features
 // Dense calls over many tiles are cut into sub-batches (default 3) that run on their own CUDA streams: the block
 // scheduler then fills the partial last wave of one sub-batch's kernel with blocks of another's (independent
 // streams, so no ordering between them) and co-schedules blocks of different kernels on an SM, which removes most
-// of the wave-quantisation loss of 512 tiles on 2-3 x 148 block slots and mixes FMA-bound with latency-bound phases.
+// of the wave-quantisation loss of 512 tiles on 2-3 x 132 block slots and mixes FMA-bound with latency-bound phases.
 int SplitParts(lyra_b200_ctx* ctx, int n, Part* parts) {
   int np = ctx->nsplit < 1 ? 1 : (ctx->nsplit > lyra_b200_ctx::kMaxSplit ? lyra_b200_ctx::kMaxSplit : ctx->nsplit);
   if (!(ctx->map_dense_n == n && ctx->active_tiles >= 64 * np)) np = 1;
@@ -753,7 +731,6 @@ int lyra_b200_create_ex(const char* model_dir, int device, int max_streams, int 
   ok = ok && cudaEventCreateWithFlags(&ctx->ev_sync, cudaEventDisableTiming | cudaEventBlockingSync) == cudaSuccess;
   if (const char* e = std::getenv("LYRA_B200_BLOCKING_SYNC")) ctx->blocking_sync = std::atoi(e) != 0;
   if (const char* e = std::getenv("LYRA_B200_SPLIT")) ctx->nsplit = std::atoi(e);
-  if (const char* e = std::getenv("LYRA_B200_DU_CLUSTER")) ctx->du_cluster = std::atoi(e) != 0;
   if (const char* e = std::getenv("LYRA_B200_DECODER_MODE")) ctx->decoder_mode = std::strcmp(e, "tensor") == 0 ? LYRA_B200_DECODER_TENSOR : LYRA_B200_DECODER_EXACT;
   ctx->stream = ctx->own_stream;
   ok = ok && DevAlloc(&ctx->d_blob, ctx->spec.blob.size()) == cudaSuccess;
@@ -820,7 +797,7 @@ int lyra_b200_create_ex(const char* model_dir, int device, int max_streams, int 
     if (ok) for (size_t i = 0; i < P; ++i) ctx->h_slot_of[b][i] = -1;
   }
   if (ok) ok = kS == 16 ? SetSmemLimits<16>() : SetSmemLimits<8>();
-  if (ok) ok = LYRA_SET_MAX_SMEM(DecoderKernelDU, DecDU::kSmemBytes) == 0;
+  if (ok) ok = LYRA_SET_MAX_SMEM(DecoderKernelDW, DecDW::kSmemBytes) == 0;
   if (!ok) {
     g_create_error = std::string("CUDA allocation / setup failed: ") + cudaGetErrorString(cudaGetLastError());
     lyra_b200_destroy(ctx);

@@ -57,7 +57,7 @@ __device__ __forceinline__ float2 LoadFrag(const float2* p) {
 }
 
 // register prefetch depth (k-steps) of the int8 B fragments that GemmI8Mma takes straight from L2.  Deeper prefetch spills a few
-// registers at 80 per thread; measured: kernel B gains with 4 (0.294 -> 0.283 ms), kernel C loses (0.221 -> 0.254 ms)
+// registers at 80 per thread; before the H100 port kernel B gained with 4 and kernel C lost (not re-measured on the H100)
 #ifndef LYRA_I8_PD
 #define LYRA_I8_PD 2
 #endif
@@ -267,14 +267,12 @@ __device__ __forceinline__ void GemmF32Tap(const float* A, int ldA, int rowA0, i
     const int t_out = active ? mg / MGS : 0, s0 = active ? (mg % MGS) * TM : 0, n0 = active ? ng * TN : 0;
     const int g = n0 / CoutG;
     const float* Abase = A + (size_t)(g * CinG) * ldA + (rowA0 + t_out * row_stride) * S + s0;
-    // Accumulators are kept as float2 pairs of neighbouring streams: one packed FFMA2 (fma.rn.f32x2, sm_100) per pair and channel.
-    // Each half is an IEEE round-to-nearest fma of its own lane, so the fmaf-chain contract (and bit-exactness) is unchanged; the
-    // packed form halves the issue slots of the inner product.
-    float2 acc2[TM / 2][TN];
+    // One IEEE round-to-nearest fma per (stream, channel) and k, in k order: the oracle's fmaf chain, bit for bit.
+    float acc[TM][TN];
 #pragma unroll
-    for (int i = 0; i < TM / 2; ++i)
+    for (int i = 0; i < TM; ++i)
 #pragma unroll
-      for (int j = 0; j < TN; ++j) acc2[i][j] = make_float2(0.0f, 0.0f);
+      for (int j = 0; j < TN; ++j) acc[i][j] = 0.0f;
 
     if (!busy) cg += nchunks;
     for (int c = 0; busy && c < nchunks; ++c, ++cg) {
@@ -299,13 +297,12 @@ __device__ __forceinline__ void GemmF32Tap(const float* A, int ldA, int rowA0, i
         const float* wp = wcur + n0;
 #pragma unroll 4
         for (int kk = 0; kk < KC; ++kk) {
-          float2 a2[TM / 2];
+          float a[TM];
           float w[TN];
 #pragma unroll
           for (int i = 0; i < TM; i += 4) {
             const float4 v = *reinterpret_cast<const float4*>(Ap + i);
-            a2[i / 2] = make_float2(v.x, v.y);
-            a2[i / 2 + 1] = make_float2(v.z, v.w);
+            a[i] = v.x; a[i + 1] = v.y; a[i + 2] = v.z; a[i + 3] = v.w;
           }
           if (TN % 4 == 0) {
 #pragma unroll
@@ -324,11 +321,9 @@ __device__ __forceinline__ void GemmF32Tap(const float* A, int ldA, int rowA0, i
             for (int j = 0; j < TN; ++j) w[j] = wp[j];
           }
 #pragma unroll
-          for (int j = 0; j < TN; ++j) {
-            const float2 w2 = make_float2(w[j], w[j]);
+          for (int j = 0; j < TN; ++j)
 #pragma unroll
-            for (int i = 0; i < TM / 2; ++i) acc2[i][j] = __ffma2_rn(a2[i], w2, acc2[i][j]);
-          }
+            for (int i = 0; i < TM; ++i) acc[i][j] = __fmaf_rn(a[i], w[j], acc[i][j]);
           Ap += astep;
           wp += N;
         }
@@ -339,11 +334,6 @@ __device__ __forceinline__ void GemmF32Tap(const float* A, int ldA, int rowA0, i
         else lyra_mbar_arrive(&pipe->empty[set][st]);
       }
     }
-    float acc[TM][TN];
-#pragma unroll
-    for (int i = 0; i < TM / 2; ++i)
-#pragma unroll
-      for (int j = 0; j < TN; ++j) { acc[2 * i][j] = acc2[i][j].x; acc[2 * i + 1][j] = acc2[i][j].y; }
     lyra_fence_proxy_async();   // this thread's earlier stores to buffers the next ring may alias, before the bulk copies below
     __syncthreads();   // every thread is past the K loop: A may be overwritten, the weight ring reused
     if (wt0 + NT / 32 >= map.nwt && threadIdx.x == 0) {

@@ -97,11 +97,11 @@ std::vector<float> PackMmaBTf32(const std::vector<float>& b, int K, int N) {
   return out;
 }
 
-// One chunk of the UMMA decoder's weight stream (net_params.h kDuChunkBytes): elem(row, k) for row < rows, k < kc as
+// One chunk of the tensor-core decoder's weight stream (net_params.h kDuChunkBytes): elem(row, k) for row < rows, k < kc as
 // [hi part][lo part], each [kc/4][rows/8][8][4] floats.
 template <typename Elem>
-void AppendDuChunk(std::vector<uint8_t>* out, int rows, int kc, Elem elem, bool raw = false) {
-  SPEC_CHECK(kc % 8 == 0 && rows % 8 == 0 && (size_t)2 * kc * rows * 4 <= (size_t)kDuChunkBytes, "UMMA weight chunk shape");
+void AppendDuChunk(std::vector<uint8_t>* out, int rows, int kc, Elem elem) {
+  SPEC_CHECK(kc % 8 == 0 && rows % 8 == 0 && (size_t)2 * kc * rows * 4 <= (size_t)kDuChunkBytes, "tensor-core weight chunk shape");
   std::vector<float> part((size_t)2 * kc * rows, 0.0f);
   for (int k = 0; k < kc; ++k)
     for (int n = 0; n < rows; ++n) {
@@ -113,23 +113,17 @@ void AppendDuChunk(std::vector<uint8_t>* out, int rows, int kc, Elem elem, bool 
       std::memcpy(&hi, &bits, 4);
       const float lo = x - hi;                                   // exact in fp32
       const size_t idx = ((size_t)(k / 4) * (rows / 8) + n / 8) * 32 + (size_t)(n % 8) * 4 + k % 4;
-      part[idx] = raw ? x : hi;
+      part[idx] = hi;
       part[(size_t)kc * rows + idx] = lo;
     }
   const size_t off = out->size();
-  if (raw) {                                                     // the unsplit values in the layout of the hi part: the kernel splits them
-    SPEC_CHECK((size_t)kc * rows * 4 == (size_t)kDuChunkBytes / 2 && kDuRawUp2, "raw UMMA weight chunk shape");
-    out->resize(off + kDuRawChunkBytes, 0);
-    std::memcpy(out->data() + off, part.data(), (size_t)kDuRawChunkBytes);
-    return;
-  }
   out->resize(off + kDuChunkBytes, 0);
   std::memcpy(out->data() + off, part.data(), part.size() * 4);
 }
 
 struct Net {
   bool pack_tc = false;
-  mutable std::vector<std::vector<float>> kept;   // k-major fp32 GEMM matrices in packing order (decoder: source of the UMMA chunks)     // also emit tensor-core fragment-order copies of the fp32 GEMM weights (decoder)
+  mutable std::vector<std::vector<float>> kept;   // k-major fp32 GEMM matrices in packing order (decoder: source of the tensor-core weight chunks)     // also emit tensor-core fragment-order copies of the fp32 GEMM weights (decoder)
   const TflModel& m;
   const TflSubgraph& g;
   std::vector<int> convs;   // CONV_2D / DEPTHWISE_CONV_2D / TRANSPOSE_CONV ops in graph order
@@ -515,7 +509,7 @@ DecoderParams BuildDecoder(const TflModel& m, std::vector<uint8_t>* blob) {
   n.expect_conv(n.conv(35), kTransposeConv, DType::F32, 1, 64, 64, 16);
   p.last = n.PackTconvF32(n.conv(35), 16);
   {
-    SPEC_CHECK(n.kept.size() == 8 && n.kept[0].size() == (size_t)256 * 320 && n.kept[7].size() == (size_t)256 * 16, "UMMA decoder: unexpected GEMM list");
+    SPEC_CHECK(n.kept.size() == 8 && n.kept[0].size() == (size_t)256 * 320 && n.kept[7].size() == (size_t)256 * 16, "tensor-core decoder: unexpected GEMM list");
     std::vector<uint8_t> chunks;
     const std::vector<float>& wu = n.kept[0];                 // decoder_2/simple: [(j, ci)][(r, co)], 256 x 320
     for (int mb = 0; mb < 5; ++mb)
@@ -523,16 +517,16 @@ DecoderParams BuildDecoder(const TflModel& m, std::vector<uint8_t>* blob) {
         AppendDuChunk(&chunks, 128, 16, [&](int row, int k) {
           const int m = mb * 128 + row, j = m / 320, rc = m % 320, ci = kc * 16 + k;
           return j < 2 ? wu[(size_t)(j * 128 + ci) * 320 + rc] : 0.0f;
-        }, kDuRawUp2);
+        });
     for (int g = 1; g <= 6; ++g) {
-      SPEC_CHECK(n.kept[(size_t)g].size() == (size_t)64 * 64, "UMMA decoder: residual-unit GEMM shape");
+      SPEC_CHECK(n.kept[(size_t)g].size() == (size_t)64 * 64, "tensor-core decoder: residual-unit GEMM shape");
       const std::vector<float>& w = n.kept[(size_t)g];         // [k = cin][n = cout]
       for (int kc = 0; kc < 2; ++kc) AppendDuChunk(&chunks, 64, 32, [&](int row, int k) { return w[(size_t)(kc * 32 + k) * 64 + row]; });
     }
     const std::vector<float>& wl = n.kept[7];                 // last_layer: [(tap, ci)][n], 256 x 16
     for (int kc = 0; kc < 2; ++kc)
       AppendDuChunk(&chunks, 64, 32, [&](int row, int k) { return wl[(size_t)((row / 16) * 64 + kc * 32 + k) * 16 + row % 16]; });
-    SPEC_CHECK(chunks.size() == (size_t)kDuUp2Chunks * kDuRawChunkBytes + (size_t)(kDuNumChunks - kDuUp2Chunks) * kDuChunkBytes, "UMMA decoder: chunk count");
+    SPEC_CHECK(chunks.size() == (size_t)kDuNumChunks * kDuChunkBytes, "tensor-core decoder: chunk count");
     while (blob->size() % 128) blob->push_back(0);
     p.du_chunks = Append(blob, chunks);
   }

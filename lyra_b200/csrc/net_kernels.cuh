@@ -112,7 +112,7 @@ __device__ __forceinline__ void LoadTileMeta(const TileIo& io, const int* n18_gl
 constexpr int kTileIdle = -2;
 
 // The tile's streaming state (one contiguous block per kernel, 65-190 KB; the 262 MB working set of 4096 streams does not stay
-// in the 126 MB L2 between hops) is requested into the L2 as soon as the block knows its tile: the ring / tail loads of the
+// in the 50 MB L2 between hops) is requested into the L2 as soon as the block knows its tile: the ring / tail loads of the
 // later phases then find it there instead of paying the HBM latency phase by phase.
 #ifndef LYRA_PREFETCH_STATE
 #define LYRA_PREFETCH_STATE 1
@@ -428,7 +428,7 @@ struct EncB {
   static constexpr int kStg = S <= 8 ? LYRA_BC_STAGES : kStages;      // ring depth of the kernel's fp32 GEMMs
   static constexpr int kWBytes = kMax(kStg * 8 * 256 * 4, 2 * 64 * LQ2 * 4);
   static constexpr int kI8Pd = S <= 8 ? LYRA_B_I8_PD : LYRA_I8_PD;    // k-steps of int8 weight fragments in flight from L2
-  // LYRA_B_DEEP_RINGS (experiment, off: measured slower, 0.307 vs 0.294 ms - with three blocks per SM the GEMM phases are bound by
+  // LYRA_B_DEEP_RINGS (experiment, off: slower before the H100 port - with three blocks per SM the GEMM phases are bound by
   // shared-memory operand delivery, not by the ring): the 8-32-row GEMMs' rings borrow the neighbouring regions that are dead
   // while their K loops run:
   //   encoder_1 (three units)   ring over [C | W]: hq is not written before the mixed unit      7 stages x 4 KB (8 k-rows x 128)

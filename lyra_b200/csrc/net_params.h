@@ -60,9 +60,9 @@ struct UpI8 {
   uint32_t bias_f32[4];     // the f32 constants subtracted from the overlap tails (SUB ops), [64] each
 };
 
-// Kernel D's GEMM weights for the tcgen05 (UMMA) decoder: kDuNumChunks chunks of kDuChunkBytes.  A chunk is a [rows x kc]
-// slice of one layer's weight operand, split into hi + lo (hi = the 19 bits a TF32 operand keeps, lo = x - hi) and stored as
-// [hi part][lo part], each part in the K-major no-swizzle core-matrix layout [kc/4][rows/8][8 rows][4 k] that a UMMA
+// Kernel D's GEMM weights for the tensor-core decoder (DecoderKernelDW): kDuNumChunks chunks of kDuChunkBytes.  A chunk is a
+// [rows x kc] slice of one layer's weight operand, split into hi + lo (hi = the 19 bits a TF32 operand keeps, lo = x - hi) and
+// stored as [hi part][lo part], each part in the K-major no-swizzle core-matrix layout [kc/4][rows/8][8 rows][4 k] that a wgmma
 // shared-memory descriptor addresses with LBO = (rows/8) * 128 bytes and SBO = 128 bytes.  One chunk = one bulk copy = one
 // stage of the kernel's weight ring.
 //   chunks  0..39  decoder_2/simple, as the A operand (the GEMM is computed transposed: weights are the rows, the 32
@@ -72,13 +72,6 @@ struct UpI8 {
 //   chunks 52..53  last_layer as ONE 64 x 64 GEMM: B row = tap * 16 + n (n = output sample within the stride), k = cin;
 //                  the four taps are summed across time rows in the epilogue
 constexpr int kDuChunkBytes = 16384;
-// LYRA_DU_RAW=1 (experiment, off): decoder_2/simple's chunks travel as plain fp32 - the hi half of a stage - and are split into
-// hi | lo in shared memory by the kernel's row warps; by default every chunk is stored pre-split
-#ifndef LYRA_DU_RAW
-#define LYRA_DU_RAW 0
-#endif
-constexpr bool kDuRawUp2 = LYRA_DU_RAW != 0;
-constexpr int kDuRawChunkBytes = kDuRawUp2 ? kDuChunkBytes / 2 : kDuChunkBytes;   // bytes of one decoder_2/simple chunk in the blob
 constexpr int kDuNumChunks = 54;
 constexpr int kDuUp2Chunks = 40, kDuUnitChunk0 = 40, kDuLastChunk0 = 52;
 
@@ -97,7 +90,7 @@ struct DecoderParams {
   GemmF32 up2;              // decoder_2/simple: transposed K=10 s=5, 128 -> 64; weights [(j,ci)][(r,co)], bias [64]
   ResF32 r2[3];             // decoder_2/resnet_*: 64 ch
   GemmF32 last;             // last_layer: transposed K=64 s=16, 64 -> 1; weights [(j,ci)][r], bias [1]
-  uint32_t du_chunks;       // the UMMA decoder's weight chunks (see kDuChunkBytes)
+  uint32_t du_chunks;       // the tensor-core decoder's weight chunks (see kDuChunkBytes)
   int32_t zp_state[3];      // int8 ring zero points: m_dw ring, q[0], q[1]
 };
 

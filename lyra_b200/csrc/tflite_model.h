@@ -1,6 +1,6 @@
 // Product-side weight/graph loader: a dependency-free reader for the three TFLite flatbuffers that
 // the reference hands to tflite::FlatBufferModel::BuildFromFile (lyra/tflite_model_wrapper.cc:39-44).
-// Replaces TfLiteModelWrapper::Create's model loading for the B200 path; the graphs themselves are
+// Replaces TfLiteModelWrapper::Create's model loading for the CUDA path; the graphs themselves are
 // never interpreted on the product side — model_spec.cc pattern-matches them into fused layers.
 #pragma once
 

@@ -6,7 +6,7 @@
  *   lyra/model_coeffs/lyragan.tflite               (reference call site: lyra/lyra_gan_model.cc:53-64)
  * which the reference executes with tflite::Interpreter::Invoke (lyra/tflite_model_wrapper.cc:102-104).
  * TensorFlow Lite v2.11.0 (commit d5b57ca93e506df258271ea00fc29cf98383a374, reference WORKSPACE:168-174)
- * is NOT vendored in /root/reference, so each builtin op is restated here from TFLite's published
+ * is NOT vendored in the reference repository, so each builtin op is restated here from TFLite's published
  * *reference kernels* (tensorflow/lite/kernels/internal/reference/{conv,depthwiseconv_float,
  * transpose_conv,leaky_relu,add,sub,quantize,dequantize,concatenation,strided_slice}.h and
  * reference/integer_ops/{conv,depthwise_conv,transpose_conv,add}.h), including the gemmlowp

@@ -17,7 +17,7 @@ EMU_SO = os.path.join(EMU_DIR, "_build", "liblyra_b200_emu.so")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100: run with -m gpu)")
 
 
 def read_wav(name):

@@ -82,7 +82,6 @@ void launch(dim3 grid, dim3 block, size_t smem_bytes, const std::function<void()
         g_blockIdx = uint3_emu{bx, by, bz};
         std::memset(b.smem, 0xCD, smem_bytes);   // poison: uninitialised shared memory shows up as garbage
         std::memset(b.static_smem, 0, sizeof(b.static_smem));
-        b.tmem_used = 0;
         b.arrived = 0;
         b.done = 0;
         for (unsigned w = 0; w < nwarps; ++w) {

@@ -64,8 +64,6 @@ struct BlockState {
   uint32_t warp_scratch[64][32][8];
   char* smem = nullptr;
   alignas(16) char static_smem[512];   // storage for the product's function-local __shared__ objects (zeroed per block)
-  std::vector<float> tmem;             // tensor memory: 128 lanes x 512 columns of 32-bit cells (allocated on first use)
-  unsigned tmem_used = 0;              // columns handed out by the emulated tcgen05.alloc
   std::function<void()> body;
 };
 
@@ -123,7 +121,6 @@ static inline unsigned __ballot_sync(unsigned, int pred) {
 }
 
 static inline float __fmaf_rn(float a, float b, float c) { return std::fmaf(a, b, c); }
-static inline float2 __ffma2_rn(float2 a, float2 b, float2 c) { return float2{std::fmaf(a.x, b.x, c.x), std::fmaf(a.y, b.y, c.y)}; }
 static inline float __fadd_rn(float a, float b) { volatile float r = a + b; return r; }
 static inline float __fsub_rn(float a, float b) { volatile float r = a - b; return r; }
 static inline float __fmul_rn(float a, float b) { volatile float r = a * b; return r; }

@@ -1,4 +1,4 @@
-"""GPU tier (B200): parity tests proper, through the C ABI of the nvcc-built library, against the oracle on the
+"""GPU tier (H100): parity tests proper, through the C ABI of the nvcc-built library, against the oracle on the
 same seeded inputs; plus size-independent properties at BASELINE.json's full sizes."""
 import json
 import os
@@ -342,22 +342,19 @@ def test_cpp_duplex_server_example(gpu_api, oracle, tmp_path):
     print(big.stdout.strip())
 
 
-@pytest.mark.parametrize("probe,cases", [("umma_probe", 2), ("umma_probe2", 7)])
-def test_umma_probes_on_hardware(tmp_path, probe, cases):
-    """tests/cpp/umma_probe{,2}.cu built with nvcc: the tcgen05 / TMEM instruction sequences of device_compat.h that the product's
-    UMMA kernel (DecoderKernelDU) is made of - shared-memory descriptors, split-precision TF32 MMAs, A operands in tensor memory,
-    tcgen05.st / wide tcgen05.ld, kind::i8, N = 160 / 16 shapes, bulk stores.  The product depends on them: a mismatch is a failure."""
-    import shutil
+def test_wgmma_probe_on_hardware(tmp_path):
+    """tests/cpp/wgmma_probe.cu built with nvcc: the wgmma instruction sequences of device_compat.h that the product's tensor-core
+    decoder kernel (DecoderKernelDW) is made of - shared-memory descriptors, register A operands, fragment layouts, split-precision
+    TF32 MMAs, the accumulator-to-operand shuffle.  The product depends on them: a mismatch is a failure."""
     import subprocess
+    import __graft_entry__ as g
     from conftest import ROOT
-    if shutil.which("nvcc") is None:
-        pytest.skip("nvcc not available on this box")
-    exe = str(tmp_path / probe)
-    subprocess.check_call(["nvcc", "-gencode", "arch=compute_100a,code=sm_100a", "-std=c++17", "-I" + os.path.join(ROOT, "lyra_b200", "csrc"),
-                           "-o", exe, os.path.join(ROOT, "tests", "cpp", probe + ".cu")])
+    exe = str(tmp_path / "wgmma_probe")
+    subprocess.check_call([g.NVCC, "-gencode", "arch=compute_90a,code=sm_90a", "-std=c++17", "-I" + os.path.join(ROOT, "lyra_b200", "csrc"),
+                           "-o", exe, os.path.join(ROOT, "tests", "cpp", "wgmma_probe.cu")])
     out = subprocess.run(["timeout", "60", exe], capture_output=True, text=True, timeout=120)
     print(out.stdout.strip())
-    assert out.returncode == 0 and out.stdout.count("MATCH") == cases and "MISMATCH" not in out.stdout, out.stdout + out.stderr
+    assert out.returncode == 0 and out.stdout.count("MATCH") == 2 and "MISMATCH" not in out.stdout, out.stdout + out.stderr
 
 
 # ---- packet-loss concealment, comfort noise, DTX (SURVEY.md section 8 rows f2, f4) ----

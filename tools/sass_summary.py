@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Per-kernel SASS evidence for profiles/: resource usage, opcode histogram, and the instructions that prove which
-hardware path a kernel uses (UTC*MMA / LDTM / STTM = tcgen05 + TMEM, UBLKCP = TMA bulk copies, SYNCS = mbarriers,
-IMMA / HMMA = legacy mma.sync, FFMA2 = packed fp32 FMA).  Runs cuobjdump on the built library (no GPU needed).
+hardware path a kernel uses (HGMMA = wgmma, UBLKCP = TMA bulk copies, SYNCS = mbarriers,
+IMMA / HMMA = mma.sync).  Runs cuobjdump on the built library (no GPU needed).
 
 usage: tools/sass_summary.py <tag>          -> profiles/<tag>_sass_<kernel>.txt
 """
@@ -14,14 +14,14 @@ import sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 LIB = os.path.join(ROOT, "lyra_b200", "liblyra_b200.so")
 
-# headline instantiations (8-stream tiles; DecoderKernelC<8,true> feeds DecoderKernelDU in the tensor mode)
+# headline instantiations (8-stream tiles; DecoderKernelC<8,true> feeds DecoderKernelDW in the tensor mode)
 KERNELS = {
     "EncoderKernelA": r"EncoderKernelAILi8E",
     "EncoderKernelB": r"EncoderKernelBILi8E",
     "DecoderKernelC_tensor": r"DecoderKernelCILi8ELb1E",
     "DecoderKernelC_exact": r"DecoderKernelCILi8ELb0E",
     "DecoderKernelD_exact": r"DecoderKernelDILi8ELb0E",
-    "DecoderKernelDU": r"DecoderKernelDUE",
+    "DecoderKernelDW": r"DecoderKernelDWE",
     "RvqEncodeKernel": r"RvqEncodeKernelE",
     "RvqDecodeKernel": r"RvqDecodeKernelE",
     "LogMelKernel": r"LogMelKernelE",
@@ -31,9 +31,8 @@ KERNELS = {
     "PlcPlanKernel": r"PlcPlanKernelE",
     "ResampleKernel": r"ResampleKernelE",
 }
-PROOF = ("UTCHMMA", "UTCIMMA", "UTCQMMA", "UTCOMMA", "UTCMMA", "LDTM", "STTM", "UTCBAR", "UTCATOMSWS", "UBLKCP", "UTMALDG",
-         "SYNCS", "IMMA", "HMMA", "FFMA2", "BAR", "DFMA", "CALL")
-FULL_LISTING = ("DecoderKernelDU",)      # small enough to commit whole (instruction text only)
+PROOF = ("HGMMA", "WARPGROUP", "UBLKCP", "UTMALDG", "SYNCS", "IMMA", "HMMA", "BAR", "DFMA", "CALL")
+FULL_LISTING = ("DecoderKernelDW",)      # small enough to commit whole (instruction text only)
 
 
 def main():
@@ -67,7 +66,7 @@ def main():
             t = text.split()
             op = t[1] if t[0].startswith("@") and len(t) > 1 else t[0]
             hist[op.split(".")[0]] += 1
-        out = [f"# {name}: {mangled}", f"# library: lyra_b200/liblyra_b200.so (nvcc -gencode arch=compute_100a,code=sm_100a), cuobjdump -sass",
+        out = [f"# {name}: {mangled}", f"# library: lyra_b200/liblyra_b200.so (nvcc -gencode arch=compute_90a,code=sm_90a), cuobjdump -sass",
                f"# resources: {usage.get(mangled, '?')}", f"# instructions: {len(insts)}", "", "## opcode histogram"]
         for op, n in hist.most_common():
             out.append(f"{n:8d}  {op}")
@@ -85,7 +84,7 @@ def main():
         path = os.path.join(ROOT, "profiles", f"{tag}_sass_{name}.txt")
         with open(path, "w") as f:
             f.write("\n".join(out) + "\n")
-        print(path, len(insts), {p: hist[p] for p in ("UTCHMMA", "LDTM", "STTM", "UBLKCP", "IMMA", "HMMA", "FFMA2", "FFMA") if hist[p]})
+        print(path, len(insts), {p: hist[p] for p in ("HGMMA", "UBLKCP", "IMMA", "HMMA", "FFMA") if hist[p]})
 
 
 if __name__ == "__main__":
