@@ -54,6 +54,7 @@ void lyra_b200_destroy(lyra_b200_ctx* ctx);
 /* Human-readable reason of the last failure on this context (or of the last failed create when ctx is NULL). */
 const char* lyra_b200_last_error(const lyra_b200_ctx* ctx);
 int lyra_b200_max_streams(const lyra_b200_ctx* ctx);
+/* Streams per tile, the unit of work of one thread block in the conv-net kernels: 8 (0 when ctx is NULL). */
 int lyra_b200_tile_streams(const lyra_b200_ctx* ctx);
 
 /* Replaces TfLiteModelWrapper::ResetVariableTensors (lyra/tflite_model_wrapper.cc:111-113) per stream:

@@ -45,7 +45,6 @@ std::string g_create_error;
 struct lyra_b200_ctx {
   ModelSpec spec;
   int device = 0, max_streams = 0, ntiles = 0, padded = 0;
-  int S = 8;                // streams per tile (8: two blocks per SM; 16: one)
   int roles = LYRA_B200_ROLE_ENCODER | LYRA_B200_ROLE_DECODER;   // which halves of the streaming state this context holds
   uint8_t* d_blob = nullptr;
   // streaming state, one block per kernel
@@ -223,7 +222,7 @@ int PrepareMap(lyra_b200_ctx* ctx, const int32_t* ids, int n) {
   // tiles in order of first appearance
   if (++ctx->map_gen == 0) { std::fill(ctx->tile_gen.begin(), ctx->tile_gen.end(), 0u); ctx->map_gen = 1; }
   for (int k = 0; k < n; ++k) {
-    const int t = (ids ? ids[k] : k) / ctx->S;
+    const int t = (ids ? ids[k] : k) / kTileStreams;
     if (ctx->tile_gen[(size_t)t] != ctx->map_gen) { ctx->tile_gen[(size_t)t] = ctx->map_gen; tile_list[ntl++] = t; }
   }
   ctx->active_tiles = ntl;
@@ -244,21 +243,17 @@ struct Part {
 };
 Part WholeCall(lyra_b200_ctx* ctx, int n) { return Part{0, ctx->active_tiles, 0, n, ctx->stream}; }
 
-template <int kS>
-int LaunchEncoderNetsT(lyra_b200_ctx* ctx, const Part& p, const int16_t* d_pcm, float* d_features) {
+int LaunchEncoderNets(lyra_b200_ctx* ctx, const Part& p, const int16_t* d_pcm, float* d_features) {
   const TileIo io{ctx->d_tile_list + p.tile0, ctx->d_slot_of, ctx->cur_skip};
   { ProfScope ps(ctx, 0, p.st);
-  LYRA_LAUNCH(EncoderKernelA<kS>, dim3((unsigned)p.ntiles), dim3(EncA<kS>::NT), (size_t)EncA<kS>::kSmemBytes, p.st,
+  LYRA_LAUNCH(EncoderKernelA, dim3((unsigned)p.ntiles), dim3(EncA::NT), (size_t)EncA::kSmemBytes, p.st,
               ctx->d_blob, ctx->spec.enc, io, d_pcm, reinterpret_cast<float*>(ctx->d_state[0]), ctx->d_n18[0], ctx->d_mid_enc); }
   { ProfScope ps(ctx, 1, p.st);
-  LYRA_LAUNCH(EncoderKernelB<kS>, dim3((unsigned)p.ntiles), dim3(EncB<kS>::NT), (size_t)EncB<kS>::kSmemBytes, p.st,
+  LYRA_LAUNCH(EncoderKernelB, dim3((unsigned)p.ntiles), dim3(EncB::NT), (size_t)EncB::kSmemBytes, p.st,
               ctx->d_blob, ctx->spec.enc, io, ctx->d_mid_enc, reinterpret_cast<float*>(ctx->d_state[1]), ctx->d_n18[1], d_features); }
   ctx->launches += 2;
   CU(cudaGetLastError());
   return LYRA_B200_OK;
-}
-int LaunchEncoderNets(lyra_b200_ctx* ctx, const Part& p, const int16_t* d_pcm, float* d_features) {
-  return ctx->S == 16 ? LaunchEncoderNetsT<16>(ctx, p, d_pcm, d_features) : LaunchEncoderNetsT<8>(ctx, p, d_pcm, d_features);
 }
 
 int LaunchQuantize(lyra_b200_ctx* ctx, const Part& p, const float* d_features, int num_bits, uint8_t* d_packets, int* d_indices,
@@ -286,41 +281,32 @@ int LaunchDequantize(lyra_b200_ctx* ctx, const Part& p, const uint8_t* d_packets
   return LYRA_B200_OK;
 }
 
-template <int kS, bool kTC>
-int LaunchDecoderNetsT(lyra_b200_ctx* ctx, const Part& p, const float* d_features, int16_t* d_pcm) {
-  const TileIo io{ctx->d_tile_list + p.tile0, ctx->d_slot_of, ctx->cur_skip};
-  using LC = DecC<kS, kTC>;
-  using LD = DecD<kS, kTC>;
-  { ProfScope ps(ctx, 4, p.st);
-  LYRA_LAUNCH((DecoderKernelC<kS, kTC>), dim3((unsigned)p.ntiles), dim3(LC::NT), (size_t)LC::kSmemBytes, p.st,
-              ctx->d_blob, ctx->spec.dec, io, d_features, reinterpret_cast<float*>(ctx->d_state[2]), ctx->d_n18[2], ctx->d_mid_dec); }
-  { ProfScope ps(ctx, 5, p.st);
-  LYRA_LAUNCH((DecoderKernelD<kS, kTC>), dim3((unsigned)p.ntiles), dim3(LD::NT), (size_t)LD::kSmemBytes, p.st,
-              ctx->d_blob, ctx->spec.dec, io, ctx->d_mid_dec, reinterpret_cast<float*>(ctx->d_state[3]), ctx->d_n18[3], d_pcm); }
-  ctx->launches += 2;
-  CU(cudaGetLastError());
-  return LYRA_B200_OK;
-}
-// Tensor mode at 8-stream tiles (the default tile): kernel C with its fp32 residual units on mma.sync TF32, kernel D on warpgroup
-// MMAs (wgmma, A operands and accumulators in registers; net_kernels_wgmma.cuh).
-int LaunchDecoderNetsWgmma(lyra_b200_ctx* ctx, const Part& p, const float* d_features, int16_t* d_pcm) {
-  const TileIo io{ctx->d_tile_list + p.tile0, ctx->d_slot_of, ctx->cur_skip};
-  using LC = DecC<8, true>;
-  { ProfScope ps(ctx, 4, p.st);
-  LYRA_LAUNCH((DecoderKernelC<8, true>), dim3((unsigned)p.ntiles), dim3(LC::NT), (size_t)LC::kSmemBytes, p.st,
-              ctx->d_blob, ctx->spec.dec, io, d_features, reinterpret_cast<float*>(ctx->d_state[2]), ctx->d_n18[2], ctx->d_mid_dec); }
-  { ProfScope ps(ctx, 5, p.st);
-  LYRA_LAUNCH(DecoderKernelDW, dim3((unsigned)p.ntiles), dim3(DecDW::NT), (size_t)DecDW::kSmemBytes, p.st,
-              ctx->d_blob, ctx->spec.dec, io, ctx->d_mid_dec, reinterpret_cast<float*>(ctx->d_state[3]), ctx->d_n18[3], d_pcm); }
-  ctx->launches += 2;
-  CU(cudaGetLastError());
-  return LYRA_B200_OK;
-}
+// Exact mode: DecoderKernelC<false> + DecoderKernelD, fp32 FMA chains bit-exact with the oracle.  Tensor mode: DecoderKernelC<true>
+// (decoder_1's 1x1 convolutions on mma.sync TF32) + DecoderKernelDW (warpgroup MMAs, A operands and accumulators in registers;
+// net_kernels_wgmma.cuh).
 int LaunchDecoderNets(lyra_b200_ctx* ctx, const Part& p, const float* d_features, int16_t* d_pcm) {
+  const TileIo io{ctx->d_tile_list + p.tile0, ctx->d_slot_of, ctx->cur_skip};
   const bool tc = ctx->decoder_mode == LYRA_B200_DECODER_TENSOR;
-  if (tc && ctx->S == 8) return LaunchDecoderNetsWgmma(ctx, p, d_features, d_pcm);
-  if (ctx->S == 16) return tc ? LaunchDecoderNetsT<16, true>(ctx, p, d_features, d_pcm) : LaunchDecoderNetsT<16, false>(ctx, p, d_features, d_pcm);
-  return tc ? LaunchDecoderNetsT<8, true>(ctx, p, d_features, d_pcm) : LaunchDecoderNetsT<8, false>(ctx, p, d_features, d_pcm);
+  const dim3 grid((unsigned)p.ntiles);
+  float* st_c = reinterpret_cast<float*>(ctx->d_state[2]);
+  float* st_d = reinterpret_cast<float*>(ctx->d_state[3]);
+  { ProfScope ps(ctx, 4, p.st);
+  if (tc)
+    LYRA_LAUNCH(DecoderKernelC<true>, grid, dim3(DecC<true>::NT), (size_t)DecC<true>::kSmemBytes, p.st,
+                ctx->d_blob, ctx->spec.dec, io, d_features, st_c, ctx->d_n18[2], ctx->d_mid_dec);
+  else
+    LYRA_LAUNCH(DecoderKernelC<false>, grid, dim3(DecC<false>::NT), (size_t)DecC<false>::kSmemBytes, p.st,
+                ctx->d_blob, ctx->spec.dec, io, d_features, st_c, ctx->d_n18[2], ctx->d_mid_dec); }
+  { ProfScope ps(ctx, 5, p.st);
+  if (tc)
+    LYRA_LAUNCH(DecoderKernelDW, grid, dim3(DecDW::NT), (size_t)DecDW::kSmemBytes, p.st,
+                ctx->d_blob, ctx->spec.dec, io, ctx->d_mid_dec, st_d, ctx->d_n18[3], d_pcm);
+  else
+    LYRA_LAUNCH(DecoderKernelD, grid, dim3(DecD::NT), (size_t)DecD::kSmemBytes, p.st,
+                ctx->d_blob, ctx->spec.dec, io, ctx->d_mid_dec, st_d, ctx->d_n18[3], d_pcm); }
+  ctx->launches += 2;
+  CU(cudaGetLastError());
+  return LYRA_B200_OK;
 }
 
 // Dense calls over many tiles are cut into sub-batches (default 3) that run on their own CUDA streams: the block
@@ -333,7 +319,7 @@ int SplitParts(lyra_b200_ctx* ctx, int n, Part* parts) {
   if (np == 1) { parts[0] = WholeCall(ctx, n); return 1; }
   for (int i = 0; i < np; ++i) {
     const int t0 = (int)((long long)ctx->active_tiles * i / np), t1 = (int)((long long)ctx->active_tiles * (i + 1) / np);
-    const int s0 = t0 * ctx->S, s1 = i + 1 == np ? n : t1 * ctx->S;
+    const int s0 = t0 * kTileStreams, s1 = i + 1 == np ? n : t1 * kTileStreams;
     parts[i] = Part{t0, t1 - t0, s0, s1 - s0, i == 0 ? ctx->stream : ctx->aux_stream[i - 1]};
   }
   return np;
@@ -502,13 +488,10 @@ int UploadIds(lyra_b200_ctx* ctx, const int32_t* ids, int n, const int** d_ids) 
   return LYRA_B200_OK;
 }
 
-template <int kS>
 bool SetSmemLimits() {
-  return LYRA_SET_MAX_SMEM(EncoderKernelA<kS>, EncA<kS>::kSmemBytes) == 0 && LYRA_SET_MAX_SMEM(EncoderKernelB<kS>, EncB<kS>::kSmemBytes) == 0 &&
-         LYRA_SET_MAX_SMEM((DecoderKernelC<kS, false>), (DecC<kS, false>::kSmemBytes)) == 0 &&
-         LYRA_SET_MAX_SMEM((DecoderKernelD<kS, false>), (DecD<kS, false>::kSmemBytes)) == 0 &&
-         LYRA_SET_MAX_SMEM((DecoderKernelC<kS, true>), (DecC<kS, true>::kSmemBytes)) == 0 &&
-         LYRA_SET_MAX_SMEM((DecoderKernelD<kS, true>), (DecD<kS, true>::kSmemBytes)) == 0;
+  return LYRA_SET_MAX_SMEM(EncoderKernelA, EncA::kSmemBytes) == 0 && LYRA_SET_MAX_SMEM(EncoderKernelB, EncB::kSmemBytes) == 0 &&
+         LYRA_SET_MAX_SMEM(DecoderKernelC<false>, DecC<false>::kSmemBytes) == 0 && LYRA_SET_MAX_SMEM(DecoderKernelD, DecD::kSmemBytes) == 0 &&
+         LYRA_SET_MAX_SMEM(DecoderKernelC<true>, DecC<true>::kSmemBytes) == 0 && LYRA_SET_MAX_SMEM(DecoderKernelDW, DecDW::kSmemBytes) == 0;
 }
 
 // initial value of every 4-byte state unit (all zero; int8 rings hold packed zero points)
@@ -546,7 +529,7 @@ int ResetImpl(lyra_b200_ctx* ctx, const int32_t* ids, int n) {
   for (int w = 0; w < 4; ++w) {
     if (!ctx->d_state[w]) continue;
     LYRA_LAUNCH(ResetStateKernel, dim3((unsigned)n), dim3(256), (size_t)0, ctx->stream,
-                ctx->d_state[w], ctx->d_init[w], ctx->units[w], ctx->S, d_ids, n, ctx->d_n18[w]);
+                ctx->d_state[w], ctx->d_init[w], ctx->units[w], kTileStreams, d_ids, n, ctx->d_n18[w]);
     ctx->launches += 1;
   }
   CU(cudaGetLastError());
@@ -706,14 +689,8 @@ int lyra_b200_create_ex(const char* model_dir, int device, int max_streams, int 
   ctx->device = device;
   ctx->max_streams = max_streams;
   ctx->roles = roles;
-  {
-    // streams per tile: 8 (default, two blocks per SM) or 16; LYRA_B200_TILE_STREAMS overrides for experiments
-    const char* e = std::getenv("LYRA_B200_TILE_STREAMS");
-    ctx->S = (e && std::atoi(e) == 16) ? 16 : 8;
-  }
-  const int kS = ctx->S;
-  ctx->ntiles = (max_streams + kS - 1) / kS;
-  ctx->padded = ctx->ntiles * kS;
+  ctx->ntiles = (max_streams + kTileStreams - 1) / kTileStreams;
+  ctx->padded = ctx->ntiles * kTileStreams;
   ctx->tile_gen.assign((size_t)ctx->ntiles, 0u);
   const size_t P = (size_t)ctx->padded;
   bool ok = cudaSetDevice(device) == cudaSuccess;
@@ -729,9 +706,6 @@ int lyra_b200_create_ex(const char* model_dir, int device, int max_streams, int 
   }
   ok = ok && cudaEventCreateWithFlags(&ctx->ev_fork, cudaEventDisableTiming) == cudaSuccess;
   ok = ok && cudaEventCreateWithFlags(&ctx->ev_sync, cudaEventDisableTiming | cudaEventBlockingSync) == cudaSuccess;
-  if (const char* e = std::getenv("LYRA_B200_BLOCKING_SYNC")) ctx->blocking_sync = std::atoi(e) != 0;
-  if (const char* e = std::getenv("LYRA_B200_SPLIT")) ctx->nsplit = std::atoi(e);
-  if (const char* e = std::getenv("LYRA_B200_DECODER_MODE")) ctx->decoder_mode = std::strcmp(e, "tensor") == 0 ? LYRA_B200_DECODER_TENSOR : LYRA_B200_DECODER_EXACT;
   ctx->stream = ctx->own_stream;
   ok = ok && DevAlloc(&ctx->d_blob, ctx->spec.blob.size()) == cudaSuccess;
   ok = ok && cudaMemcpy(ctx->d_blob, ctx->spec.blob.data(), ctx->spec.blob.size(), cudaMemcpyHostToDevice) == cudaSuccess;
@@ -743,8 +717,8 @@ int lyra_b200_create_ex(const char* model_dir, int device, int max_streams, int 
     ok = ok && cudaMemcpy(ctx->d_init[w], img.data(), img.size() * 4, cudaMemcpyHostToDevice) == cudaSuccess;
     ok = ok && DevAlloc(&ctx->d_n18[w], P) == cudaSuccess;
   }
-  if (roles & LYRA_B200_ROLE_ENCODER) ok = ok && DevAlloc(&ctx->d_mid_enc, (size_t)ctx->ntiles * 128 * 4 * kS) == cudaSuccess;
-  if (roles & LYRA_B200_ROLE_DECODER) ok = ok && DevAlloc(&ctx->d_mid_dec, (size_t)ctx->ntiles * 128 * 4 * kS) == cudaSuccess;
+  if (roles & LYRA_B200_ROLE_ENCODER) ok = ok && DevAlloc(&ctx->d_mid_enc, P * 128 * 4) == cudaSuccess;
+  if (roles & LYRA_B200_ROLE_DECODER) ok = ok && DevAlloc(&ctx->d_mid_dec, P * 128 * 4) == cudaSuccess;
   ok = ok && DevAlloc(&ctx->d_logmel_prev[0], P * 320) == cudaSuccess;
   ok = ok && DevAlloc(&ctx->d_logmel_prev[1], P * 320) == cudaSuccess;
   ok = ok && DevAlloc(&ctx->d_logmel_prev[2], P * 320) == cudaSuccess;
@@ -796,8 +770,7 @@ int lyra_b200_create_ex(const char* model_dir, int device, int max_streams, int 
     ok = ok && cudaEventCreateWithFlags(&ctx->ev_map[b], cudaEventDisableTiming) == cudaSuccess;
     if (ok) for (size_t i = 0; i < P; ++i) ctx->h_slot_of[b][i] = -1;
   }
-  if (ok) ok = kS == 16 ? SetSmemLimits<16>() : SetSmemLimits<8>();
-  if (ok) ok = LYRA_SET_MAX_SMEM(DecoderKernelDW, DecDW::kSmemBytes) == 0;
+  if (ok) ok = SetSmemLimits();
   if (!ok) {
     g_create_error = std::string("CUDA allocation / setup failed: ") + cudaGetErrorString(cudaGetLastError());
     lyra_b200_destroy(ctx);
@@ -849,7 +822,7 @@ void lyra_b200_destroy(lyra_b200_ctx* ctx) {
 
 const char* lyra_b200_last_error(const lyra_b200_ctx* ctx) { return ctx ? ctx->err.c_str() : g_create_error.c_str(); }
 int lyra_b200_max_streams(const lyra_b200_ctx* ctx) { return ctx ? ctx->max_streams : 0; }
-int lyra_b200_tile_streams(const lyra_b200_ctx* ctx) { return ctx ? ctx->S : 0; }
+int lyra_b200_tile_streams(const lyra_b200_ctx* ctx) { return ctx ? kTileStreams : 0; }
 uint64_t lyra_b200_launch_count(const lyra_b200_ctx* ctx) { return ctx ? ctx->launches : 0; }
 
 int lyra_b200_profile_enable(lyra_b200_ctx* ctx, int enable) {

@@ -15,59 +15,6 @@
 #include "device_compat.h"
 #include "net_params.h"
 
-// Weight fragments that a block reads exactly once (straight from L2 into registers).  Experiment switch LYRA_FRAG_NOALLOC: bit 0
-// (int8) / bit 1 (TF32) load them without allocating an L1 line (measured slower: co-resident blocks of the same kernel find each
-// other's fragments in the L1); + 4 loads them with the evict-last L1 policy instead.
-#ifndef LYRA_FRAG_NOALLOC
-#define LYRA_FRAG_NOALLOC 0
-#endif
-template <bool NOALLOC>
-__device__ __forceinline__ uint2 LoadFrag(const uint2* p) {
-#if defined(LYRA_EMU)
-  return *p;
-#else
-  if (NOALLOC) {
-    uint2 v;
-#if LYRA_FRAG_NOALLOC >= 4
-    asm volatile("ld.global.nc.L1::evict_last.v2.u32 {%0, %1}, [%2];\n" : "=r"(v.x), "=r"(v.y) : "l"(p));
-#else
-    asm volatile("ld.global.nc.L1::no_allocate.v2.u32 {%0, %1}, [%2];\n" : "=r"(v.x), "=r"(v.y) : "l"(p));
-#endif
-    return v;
-  }
-  return __ldg(p);
-#endif
-}
-template <bool NOALLOC>
-__device__ __forceinline__ float2 LoadFrag(const float2* p) {
-#if defined(LYRA_EMU)
-  return *p;
-#else
-  if (NOALLOC) {
-    float2 v;
-#if LYRA_FRAG_NOALLOC >= 4
-    asm volatile("ld.global.nc.L1::evict_last.v2.f32 {%0, %1}, [%2];\n" : "=f"(v.x), "=f"(v.y) : "l"(p));
-#else
-    asm volatile("ld.global.nc.L1::no_allocate.v2.f32 {%0, %1}, [%2];\n" : "=f"(v.x), "=f"(v.y) : "l"(p));
-#endif
-    return v;
-  }
-  return __ldg(p);
-#endif
-}
-
-// register prefetch depth (k-steps) of the int8 B fragments that GemmI8Mma takes straight from L2.  Deeper prefetch spills a few
-// registers at 80 per thread; before the H100 port kernel B gained with 4 and kernel C lost (not re-measured on the H100)
-#ifndef LYRA_I8_PD
-#define LYRA_I8_PD 2
-#endif
-#ifndef LYRA_B_I8_PD
-#define LYRA_B_I8_PD 4
-#endif
-#ifndef LYRA_C_I8_PD
-#define LYRA_C_I8_PD 2
-#endif
-
 namespace lyra_b200 {
 
 template <typename T>
@@ -358,7 +305,11 @@ __device__ __forceinline__ void GemmF32Tap(const float* A, int ldA, int rowA0, i
 //   A warp owns one 16-row m-tile (rows m = t*S + s) and NTW consecutive 8-column n-tiles.
 //   epi(t, s, n4, acc) is called per output row and group of 4 consecutive channels n4..n4+3 (acc is [1][4]),
 //   after neighbouring lanes have exchanged their halves of the accumulator tile.
-template <int S, int NT, int NTW, int PDI = LYRA_I8_PD, typename Epi>
+// The fragments are loaded through the L1 (loads that skip it were slower: co-resident blocks of a kernel find each other's
+// fragments there).  Default prefetch depth: deeper prefetch spills a few registers at 80 per thread; before the H100 port
+// kernel B gained with 4 and kernel C lost (not re-measured on the H100).
+constexpr int kI8Pd = 2;
+template <int S, int NT, int NTW, int PDI = kI8Pd, typename Epi>
 __device__ __forceinline__ void GemmI8Mma(const uint32_t* A, int ldA, int rowA0, int row_stride, int ntaps, int CinG,
                                           int groups, int T_out, int N, const uint2* __restrict__ Wf, Epi epi) {
   constexpr int PD = PDI;             // register prefetch depth of the B fragments (k-steps)
@@ -384,7 +335,7 @@ __device__ __forceinline__ void GemmI8Mma(const uint32_t* A, int ldA, int rowA0,
     for (int p = 0; p < PD; ++p)
       if (p < KS) {
 #pragma unroll
-        for (int j = 0; j < NTW; ++j) bf[p][j] = LoadFrag<(LYRA_FRAG_NOALLOC & 1) != 0>(wp + p * ks_stride + j * 32);
+        for (int j = 0; j < NTW; ++j) bf[p][j] = __ldg(wp + p * ks_stride + j * 32);
       }
     for (int ks0 = 0; ks0 < KS; ks0 += PD) {
 #pragma unroll
@@ -402,7 +353,7 @@ __device__ __forceinline__ void GemmI8Mma(const uint32_t* A, int ldA, int rowA0,
           }
           if (ks + PD < KS) {
 #pragma unroll
-            for (int j = 0; j < NTW; ++j) bf[p][j] = LoadFrag<(LYRA_FRAG_NOALLOC & 1) != 0>(wp + (size_t)(ks + PD) * ks_stride + j * 32);
+            for (int j = 0; j < NTW; ++j) bf[p][j] = __ldg(wp + (size_t)(ks + PD) * ks_stride + j * 32);
           }
         }
       }
@@ -451,13 +402,10 @@ __device__ __forceinline__ void SplitTf32(float x, uint32_t& hi, uint32_t& lo) {
   lo = __float_as_uint(__fsub_rn(x, __uint_as_float(hi)));
 }
 
-#ifndef LYRA_TF32_PD
-#define LYRA_TF32_PD 8
-#endif
 template <int S, int NT, int WTM, int WTN, bool SYNC_EPI, typename Epi>
 __device__ __forceinline__ void GemmTf32Mma(const float* A, int ldA, int rowA0, int row_stride, int ntaps, int CinG,
                                             int groups, int T_out, int N, const float2* __restrict__ Wf, Epi epi) {
-  constexpr int PD = LYRA_TF32_PD;      // k-steps of B fragments in flight from L2 (registers: 2 x WTN per step)
+  constexpr int PD = 8;                 // k-steps of B fragments in flight from L2 (registers: 2 x WTN per step)
   constexpr int NW = NT / 32;
   const int lane = (int)threadIdx.x & 31, warp = (int)threadIdx.x >> 5, g = lane >> 2, t4 = lane & 3;
   const int M = T_out * S, MT = (M + 15) / 16, MTW = (MT + WTM - 1) / WTM, NTILES = N / 8, NWT = MTW * (NTILES / WTN);
@@ -493,7 +441,7 @@ __device__ __forceinline__ void GemmTf32Mma(const float* A, int ldA, int rowA0, 
     for (int p = 0; p < PD; ++p)
       if (p < KS) {
 #pragma unroll
-        for (int j = 0; j < WTN; ++j) bf[p][j] = LoadFrag<(LYRA_FRAG_NOALLOC & 2) != 0>(wp + p * ks_stride + j * 32);
+        for (int j = 0; j < WTN; ++j) bf[p][j] = __ldg(wp + p * ks_stride + j * 32);
       }
     for (int ks0 = 0; ks0 < KS; ks0 += PD) {
 #pragma unroll
@@ -524,7 +472,7 @@ __device__ __forceinline__ void GemmTf32Mma(const float* A, int ldA, int rowA0, 
           }
           if (ks + PD < KS) {
 #pragma unroll
-            for (int j = 0; j < WTN; ++j) bf[p][j] = LoadFrag<(LYRA_FRAG_NOALLOC & 2) != 0>(wp + (size_t)(ks + PD) * ks_stride + j * 32);
+            for (int j = 0; j < WTN; ++j) bf[p][j] = __ldg(wp + (size_t)(ks + PD) * ks_stride + j * 32);
           }
         }
       }

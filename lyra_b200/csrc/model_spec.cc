@@ -121,9 +121,10 @@ void AppendDuChunk(std::vector<uint8_t>* out, int rows, int kc, Elem elem) {
   std::memcpy(out->data() + off, part.data(), part.size() * 4);
 }
 
+// k-major fp32 GEMM matrices, collected in packing order (kernel D's GEMMs: the source of the tensor-core weight chunks)
+using GemmList = std::vector<std::vector<float>>;
+
 struct Net {
-  bool pack_tc = false;
-  mutable std::vector<std::vector<float>> kept;   // k-major fp32 GEMM matrices in packing order (decoder: source of the tensor-core weight chunks)     // also emit tensor-core fragment-order copies of the fp32 GEMM weights (decoder)
   const TflModel& m;
   const TflSubgraph& g;
   std::vector<int> convs;   // CONV_2D / DEPTHWISE_CONV_2D / TRANSPOSE_CONV ops in graph order
@@ -167,7 +168,8 @@ struct Net {
   }
 
   // ---- packers -------------------------------------------------------------------------------
-  GemmF32 PackConvF32(const TflOp& o) const {
+  // tf32_frags: also append the mma.sync TF32 fragment-order copy (GemmF32::wf);  gemms: if given, receives the k-major matrix
+  GemmF32 PackConvF32(const TflOp& o, bool tf32_frags = false, GemmList* gemms = nullptr) const {
     const TflTensor& w = T(w_tensor(o));
     const TflTensor& b = T(b_tensor(o));
     SPEC_CHECK(w.shape.size() == 4 && w.type == DType::F32 && b.type == DType::F32, "conv: filter rank / type");
@@ -181,13 +183,14 @@ struct Net {
           wt[((size_t)k * CinG + ci) * Cout + co] = src[((size_t)co * K + k) * CinG + ci];
     SPEC_CHECK((int)b.count() == Cout, "conv bias");
     std::vector<float> bias(b.as<float>((size_t)Cout), b.as<float>((size_t)Cout) + Cout);
-    const uint32_t wf = pack_tc && (K * CinG) % 8 == 0 && Cout % 8 == 0 ? Append(blob, PackMmaBTf32(wt, K * CinG, Cout)) : 0u;
-    if (pack_tc) kept.push_back(wt);
+    const uint32_t wf = tf32_frags ? Append(blob, PackMmaBTf32(wt, K * CinG, Cout)) : 0u;
+    if (gemms) gemms->push_back(wt);
     return GemmF32{Append(blob, wt), Append(blob, bias), wf};
   }
 
-  // transposed conv as a J-tap GEMM over (r, co) outputs: W'[(j,ci)][(r,co)] = W[co][r + s*(J-1-j)][ci]
-  GemmF32 PackTconvF32(const TflOp& o, int stride) const {
+  // transposed conv as a J-tap GEMM over (r, co) outputs: W'[(j,ci)][(r,co)] = W[co][r + s*(J-1-j)][ci]; both fp32 ones are kernel D
+  // GEMMs, so the k-major matrix also goes to `gemms`
+  GemmF32 PackTconvF32(const TflOp& o, int stride, GemmList* gemms) const {
     const TflTensor& w = T(w_tensor(o));
     const TflTensor& b = T(b_tensor(o));
     SPEC_CHECK(w.shape.size() == 4 && w.type == DType::F32 && b.type == DType::F32, "transposed conv: filter rank / type");
@@ -202,9 +205,8 @@ struct Net {
           for (int co = 0; co < Cout; ++co)
             wt[((size_t)j * Cin + ci) * N + (size_t)r * Cout + co] = src[((size_t)co * K + (r + stride * (J - 1 - j))) * Cin + ci];
     std::vector<float> bias(b.as<float>((size_t)Cout), b.as<float>((size_t)Cout) + Cout);
-    const uint32_t wf = pack_tc && (J * Cin) % 8 == 0 && N % 8 == 0 ? Append(blob, PackMmaBTf32(wt, J * Cin, N)) : 0u;
-    if (pack_tc) kept.push_back(wt);
-    return GemmF32{Append(blob, wt), Append(blob, bias), wf};
+    gemms->push_back(wt);
+    return GemmF32{Append(blob, wt), Append(blob, bias), 0u};
   }
 
   void RequantArrays(const TflTensor& x, const TflTensor& w, const TflTensor& y, int n, int repeat,
@@ -329,11 +331,12 @@ struct Net {
     return AddQ{Append(blob, l1), Append(blob, l2), m3, s3, y.zp0()};
   }
 
-  ResF32 PackResF32(int first_conv, int C, int dil, int groups2) const {
+  ResF32 PackResF32(int first_conv, int C, int dil, int groups2, bool tf32_frags = false, GemmList* gemms = nullptr) const {
     expect_conv(conv(first_conv), kDepthwiseConv2D, DType::F32, C, 3, C, 1, dil);
     expect_conv(conv(first_conv + 1), kConv2D, DType::F32, C, 1, C, 1);
     expect_conv(conv(first_conv + 2), kConv2D, DType::F32, C, 1, C / groups2, 1);
-    return ResF32{PackDwF32(conv(first_conv)), PackConvF32(conv(first_conv + 1)), PackConvF32(conv(first_conv + 2))};
+    return ResF32{PackDwF32(conv(first_conv)), PackConvF32(conv(first_conv + 1), tf32_frags, gemms),
+                  PackConvF32(conv(first_conv + 2), tf32_frags, gemms)};
   }
 
   ResI8 PackResI8(int first_conv, int C, int dil) const {
@@ -411,7 +414,6 @@ DecoderParams BuildDecoder(const TflModel& m, std::vector<uint8_t>* blob) {
   int sg = m.SignatureSubgraph("serving_default");
   if (sg < 0) sg = 0;
   Net n(m, sg, blob);
-  n.pack_tc = true;
   SPEC_CHECK(n.convs.size() == 36, "decoder: expected 36 convolution ops");
   DecoderParams p;
   std::memset(&p, 0, sizeof(p));
@@ -501,17 +503,18 @@ DecoderParams BuildDecoder(const TflModel& m, std::vector<uint8_t>* blob) {
   p.q[1] = n.PackResI8(11, 256, 9);
   p.up1 = pack_up(14, 2);
   const int dil[3] = {1, 3, 9};
-  for (int i = 0; i < 3; ++i) p.r1[i] = n.PackResF32(16 + 3 * i, 128, dil[i], 2);
+  // decoder_1's 1x1 convolutions also in TF32 fragment order: kernel C's tensor mode runs them on mma.sync (GemmTf32Mma)
+  for (int i = 0; i < 3; ++i) p.r1[i] = n.PackResF32(16 + 3 * i, 128, dil[i], 2, true);
   n.expect_conv(n.conv(25), kTransposeConv, DType::F32, 64, 10, 128, 5);
-  n.kept.clear();           // from here on: exactly kernel D's GEMMs, in order up2, (pw1, pw2) x 3, last
-  p.up2 = n.PackTconvF32(n.conv(25), 5);
-  for (int i = 0; i < 3; ++i) p.r2[i] = n.PackResF32(26 + 3 * i, 64, dil[i], 1);
+  GemmList gemms;           // kernel D's GEMMs, in order up2, (pw1, pw2) x 3, last
+  p.up2 = n.PackTconvF32(n.conv(25), 5, &gemms);
+  for (int i = 0; i < 3; ++i) p.r2[i] = n.PackResF32(26 + 3 * i, 64, dil[i], 1, false, &gemms);
   n.expect_conv(n.conv(35), kTransposeConv, DType::F32, 1, 64, 64, 16);
-  p.last = n.PackTconvF32(n.conv(35), 16);
+  p.last = n.PackTconvF32(n.conv(35), 16, &gemms);
   {
-    SPEC_CHECK(n.kept.size() == 8 && n.kept[0].size() == (size_t)256 * 320 && n.kept[7].size() == (size_t)256 * 16, "tensor-core decoder: unexpected GEMM list");
+    SPEC_CHECK(gemms.size() == 8 && gemms[0].size() == (size_t)256 * 320 && gemms[7].size() == (size_t)256 * 16, "tensor-core decoder: unexpected GEMM list");
     std::vector<uint8_t> chunks;
-    const std::vector<float>& wu = n.kept[0];                 // decoder_2/simple: [(j, ci)][(r, co)], 256 x 320
+    const std::vector<float>& wu = gemms[0];                  // decoder_2/simple: [(j, ci)][(r, co)], 256 x 320
     for (int mb = 0; mb < 5; ++mb)
       for (int kc = 0; kc < 8; ++kc)
         AppendDuChunk(&chunks, 128, 16, [&](int row, int k) {
@@ -519,11 +522,11 @@ DecoderParams BuildDecoder(const TflModel& m, std::vector<uint8_t>* blob) {
           return j < 2 ? wu[(size_t)(j * 128 + ci) * 320 + rc] : 0.0f;
         });
     for (int g = 1; g <= 6; ++g) {
-      SPEC_CHECK(n.kept[(size_t)g].size() == (size_t)64 * 64, "tensor-core decoder: residual-unit GEMM shape");
-      const std::vector<float>& w = n.kept[(size_t)g];         // [k = cin][n = cout]
+      SPEC_CHECK(gemms[(size_t)g].size() == (size_t)64 * 64, "tensor-core decoder: residual-unit GEMM shape");
+      const std::vector<float>& w = gemms[(size_t)g];          // [k = cin][n = cout]
       for (int kc = 0; kc < 2; ++kc) AppendDuChunk(&chunks, 64, 32, [&](int row, int k) { return w[(size_t)(kc * 32 + k) * 64 + row]; });
     }
-    const std::vector<float>& wl = n.kept[7];                 // last_layer: [(tap, ci)][n], 256 x 16
+    const std::vector<float>& wl = gemms[7];                  // last_layer: [(tap, ci)][n], 256 x 16
     for (int kc = 0; kc < 2; ++kc)
       AppendDuChunk(&chunks, 64, 32, [&](int row, int k) { return wl[(size_t)((row / 16) * 64 + kc * 32 + k) * 16 + row % 16]; });
     SPEC_CHECK(chunks.size() == (size_t)kDuNumChunks * kDuChunkBytes, "tensor-core decoder: chunk count");

@@ -15,28 +15,12 @@
 
 #include "kernel_prims.cuh"
 
-// resident blocks per SM the small-M kernels (B, C) are compiled for at S = 8 (their 59-72 KB of shared memory allow 3)
-#ifndef LYRA_BC_MIN_BLOCKS
-#define LYRA_BC_MIN_BLOCKS 3
-#endif
-// output channels per fp32 thread tile in the small-M layers of kernels B / C (8 streams x LYRA_BC_TN channels)
-#ifndef LYRA_B_MIN_BLOCKS
-#define LYRA_B_MIN_BLOCKS LYRA_BC_MIN_BLOCKS
-#endif
-#ifndef LYRA_C_MIN_BLOCKS
-#define LYRA_C_MIN_BLOCKS LYRA_BC_MIN_BLOCKS
-#endif
-#ifndef LYRA_BC_STAGES
-#define LYRA_BC_STAGES 3
-#endif
-#ifndef LYRA_B_DEEP_RINGS
-#define LYRA_B_DEEP_RINGS 0
-#endif
-#ifndef LYRA_BC_TN
-#define LYRA_BC_TN 4
-#endif
-
 namespace lyra_b200 {
+
+// Streams per tile: one thread block of every conv-net kernel processes one tile.  The kernels' shared-memory layouts (two
+// resident blocks per SM for A and D, three for B and C), the tile-blocked streaming state, the host's stream -> tile map and
+// DecoderKernelDW's warp-to-row mapping are all sized for it.
+constexpr int kTileStreams = 8;
 
 // Development aid (-DLYRA_PHASE_PROF): thread 0 of every block stamps clock64() at phase boundaries.
 #if defined(LYRA_PHASE_PROF) && !defined(LYRA_EMU)
@@ -111,15 +95,14 @@ __device__ __forceinline__ void LoadTileMeta(const TileIo& io, const int* n18_gl
 }
 constexpr int kTileIdle = -2;
 
+// compile-time max, for the sizes of shared-memory regions that successive layers reuse
+constexpr int kMax(int a, int b) { return a > b ? a : b; }
+
 // The tile's streaming state (one contiguous block per kernel, 65-190 KB; the 262 MB working set of 4096 streams does not stay
 // in the 50 MB L2 between hops) is requested into the L2 as soon as the block knows its tile: the ring / tail loads of the
 // later phases then find it there instead of paying the HBM latency phase by phase.
-#ifndef LYRA_PREFETCH_STATE
-#define LYRA_PREFETCH_STATE 1
-#endif
-template <int ON>
 __device__ __forceinline__ void PrefetchTileState(const void* p, int bytes) {
-  if (ON && threadIdx.x == 0) lyra_prefetch_l2(p, (unsigned)bytes);
+  if (threadIdx.x == 0) lyra_prefetch_l2(p, (unsigned)bytes);
 }
 
 // One fp32 residual unit:  d = dw(lrelu(u)); h = lrelu(pw1(d)); u' = pw2(h) + u.
@@ -211,12 +194,12 @@ __device__ __forceinline__ void ResUnitsF32x3(const uint8_t* blob, const ResF32*
 // One int8 residual unit on packed activations (quant_encoder_2/resnet_{1,2}, quant_decoder_0/resnet_{1,2}); the two
 // 1x1 convolutions run on the tensor cores.
 //   aq: LeakyReLU'd input (row offset row0a of [64][lda]); resq: the pre-activation residual; both updated in place.
-template <int S, int NT, int DIL, int PDI = LYRA_I8_PD>
+template <int S, int NT, int DIL, int PDI = kI8Pd>
 __device__ __forceinline__ void ResUnitI8(const uint8_t* blob, const ResI8& p, uint32_t* aq, int lda, int row0a,
                                           uint32_t* resq, uint32_t* dq8, uint32_t* hq, uint32_t* ring,
                                           const int* n18, const int* active, int pk, int& ph, int dil_rt = DIL) {
   constexpr int T = 2, C = 256, LD = PadLd(T * S);
-  constexpr int NTW = S >= 16 ? 8 : 4;
+  constexpr int NTW = 4;
   if (n18[S] >= 0) {
     if constexpr (DIL != 0) DwI8RingFast<S, NT, C, T, DIL>(aq, lda, row0a, dq8, LD, blob, p.dw, ring, n18[S], active);
     else if (dil_rt == 3) DwI8RingFast<S, NT, C, T, 3>(aq, lda, row0a, dq8, LD, blob, p.dw, ring, n18[S], active);
@@ -269,7 +252,7 @@ __device__ __forceinline__ void ResUnitI8(const uint8_t* blob, const ResI8& p, u
 }
 
 // quant_{en,de}coder resnet_1 and resnet_2 (dilation 3, 9; ring blocks of 6 and 18 rows back to back) as one copy of the code
-template <int S, int NT, int PDI = LYRA_I8_PD>
+template <int S, int NT, int PDI = kI8Pd>
 __device__ __forceinline__ void ResUnitsI8x2(const uint8_t* blob, const ResI8* p2, uint32_t* aq, int lda, int row0a,
                                              uint32_t* resq, uint32_t* dq8, uint32_t* hq, uint32_t* ring0,
                                              const int* n18, const int* active, int pk, int& ph) {
@@ -281,28 +264,16 @@ __device__ __forceinline__ void ResUnitsI8x2(const uint8_t* blob, const ResI8* p
 // ================================================================================================
 //                                        ENCODER  A
 // ================================================================================================
-#ifndef LYRA_A_TN
-#define LYRA_A_TN 4
-#endif
-#ifndef LYRA_A_NT
-#define LYRA_A_NT 320
-#endif
-#ifndef LYRA_A_DOWN_STAGES
-#define LYRA_A_DOWN_STAGES 5
-#endif
-#ifndef LYRA_A_DOWN_TM
-#define LYRA_A_DOWN_TM 8
-#endif
-#ifndef LYRA_A_DOWN_TN
-#define LYRA_A_DOWN_TN 4
-#endif
-template <int S>
 struct EncA {
-  static constexpr int NT = LYRA_A_NT;
-  static constexpr int TN = S >= 16 ? 8 : LYRA_A_TN;
-  static constexpr int kMinBlocks = S <= 8 ? 2 : 1;       // S = 8 tiles fit two blocks per SM
+  static constexpr int S = kTileStreams;
+  static constexpr int NT = 320;
+  static constexpr int TN = 4;
+  static constexpr int kMinBlocks = 2;
   static constexpr int LDU = 25 * S, LDD = 20 * S;
-  static constexpr int kStgDown = S <= 8 ? LYRA_A_DOWN_STAGES : kStages;   // ring depth of encoder_0/simpleconv (ring = the d buffer)
+  static constexpr int kStgDown = 5;                      // ring depth of encoder_0/simpleconv (ring = the d buffer)
+  // encoder_0/simpleconv has 4 output rows x S streams = 32 GEMM rows only: its DTM x DTN thread tiles decide how many of the
+  // block's ten warps get a tile (8 x 4: four warps)
+  static constexpr int DTM = 8, DTN = 4;
   static constexpr int kSmemU = 0;
   static constexpr int kSmemD = kSmemU + 64 * LDU * 4;
   static constexpr int kSmemW = kSmemD + 64 * LDD * 4;
@@ -311,12 +282,11 @@ struct EncA {
   static_assert(391 * S <= 64 * LDD, "first-layer input (368 rows + 23 skew rows) must fit in the d buffer");
 };
 
-template <int S>
-__global__ void __launch_bounds__(EncA<S>::NT, EncA<S>::kMinBlocks)
+__global__ void __launch_bounds__(EncA::NT, EncA::kMinBlocks)
 EncoderKernelA(const uint8_t* __restrict__ blob, EncoderParams P, TileIo io, const int16_t* __restrict__ pcm,
                float* __restrict__ state, int* __restrict__ n18g, float* __restrict__ mid) {
-  using L = EncA<S>;
-  constexpr int NT = L::NT;
+  using L = EncA;
+  constexpr int S = L::S, NT = L::NT;
   unsigned char* smem = LYRA_DYN_SMEM();
   float* u = reinterpret_cast<float*>(smem + L::kSmemU);
   float* d = reinterpret_cast<float*>(smem + L::kSmemD);
@@ -330,7 +300,7 @@ EncoderKernelA(const uint8_t* __restrict__ blob, EncoderParams P, TileIo io, con
   if (n18[S] == kTileIdle) return;
   float* st = state + (size_t)tile * EncStateA::kUnits * S;
   const int tid = (int)threadIdx.x;
-  PrefetchTileState<LYRA_PREFETCH_STATE>(st, EncStateA::kUnits * S * 4);
+  PrefetchTileState(st, EncStateA::kUnits * S * 4);
   IssuePrologue<NT>(wbuf, NextF32(BlobPtr<float>(blob, P.first.w), 16, 64, 64));
   int ph = 0;
   LYRA_PHASE(0, ph);
@@ -383,9 +353,7 @@ EncoderKernelA(const uint8_t* __restrict__ blob, EncoderParams P, TileIo io, con
     // the d buffer is free from here on: it hosts this GEMM's weight ring (kStgDown x 16 x 128 floats).  With 32 GEMM rows a chunk is
     // consumed in a fraction of the L2 round trip, so the ring is as deep as d allows.
     static_assert(L::kStgDown * 16 * 128 * 4 <= 64 * L::LDD * 4, "simpleconv weight ring must fit in d");
-    // 4 output rows x S streams = 32 GEMM rows only: LYRA_A_DOWN_TM x LYRA_A_DOWN_TN thread tiles decide how many of the block's
-    // ten warps get a tile (8 x 4: four warps; 4 x 4 or 8 x 2: eight)
-    constexpr int DTM = S >= 16 ? 8 : LYRA_A_DOWN_TM, DTN = S >= 16 ? 4 : LYRA_A_DOWN_TN;
+    constexpr int DTM = L::DTM, DTN = L::DTN;
     GemmF32Tap<S, NT, DTM, DTN, 16, 4, false, L::kStgDown>(u, L::LDU, 0, 5, 10, 64, 1, 4, 128, BlobPtr<float>(blob, P.down0.w), d, true, NoNext(),
       [&](int t, int s0, int n0, float (&acc)[DTM][DTN]) {
 #pragma unroll
@@ -403,11 +371,12 @@ EncoderKernelA(const uint8_t* __restrict__ blob, EncoderParams P, TileIo io, con
 // ================================================================================================
 //                                        ENCODER  B
 // ================================================================================================
-template <int S>
 struct EncB {
+  static constexpr int S = kTileStreams;
   static constexpr int NT = 256;
-  static constexpr int kMinBlocks = S <= 8 ? LYRA_B_MIN_BLOCKS : 1;
+  static constexpr int kMinBlocks = 3;                    // resident blocks per SM (72 KB of shared memory each)
   static constexpr int TM = 8;                            // streams per fp32 thread tile (8 x 4 tiles: fewer smem wavefronts per FMA)
+  static constexpr int TN = 4;                            // output channels per fp32 thread tile
   static constexpr int WM4 = 4 * S / TM >= 4 ? 4 : 4 * S / TM;   // m-groups per warp for T = 4 / 2 / 1 row layers
   static constexpr int WM2 = 2 * S / TM >= 4 ? 4 : 2 * S / TM;
   static constexpr int WM1 = 1 * S / TM >= 4 ? 4 : 1 * S / TM;
@@ -418,38 +387,27 @@ struct EncB {
   //   region B: d1 f32 [128][4S]  ->  u2 f32 [256][2S]
   //   region C: hq words [64][LQ2]
   //   region W: fp32 weight ring  ->  (after the last fp32 GEMM) dq8, resq words [64][LQ2] each
-  static constexpr int kMax(int a, int b) { return a > b ? a : b; }
   static constexpr int kRA = 0;
   static constexpr int kRABytes = kMax(kMax(128 * LD1 * 4, 256 * 2 * S * 4), 64 * LQA * 4 + 128 * LQB * 4);
   static constexpr int kRB = kRA + kRABytes;
   static constexpr int kRBBytes = kMax(128 * 4 * S * 4, 256 * 2 * S * 4);
   static constexpr int kRC = kRB + kRBBytes;
   static constexpr int kW = kRC + 64 * LQ2 * 4;
-  static constexpr int kStg = S <= 8 ? LYRA_BC_STAGES : kStages;      // ring depth of the kernel's fp32 GEMMs
+  // ring depth of the kernel's fp32 GEMMs.  Deeper rings, borrowing the regions that are dead during the K loops, were slower before
+  // the H100 port: with three blocks per SM the GEMM phases are bound by shared-memory operand delivery (not re-measured on the H100).
+  static constexpr int kStg = 3;
   static constexpr int kWBytes = kMax(kStg * 8 * 256 * 4, 2 * 64 * LQ2 * 4);
-  static constexpr int kI8Pd = S <= 8 ? LYRA_B_I8_PD : LYRA_I8_PD;    // k-steps of int8 weight fragments in flight from L2
-  // LYRA_B_DEEP_RINGS (experiment, off: slower before the H100 port - with three blocks per SM the GEMM phases are bound by
-  // shared-memory operand delivery, not by the ring): the 8-32-row GEMMs' rings borrow the neighbouring regions that are dead
-  // while their K loops run:
-  //   encoder_1 (three units)   ring over [C | W]: hq is not written before the mixed unit      7 stages x 4 KB (8 k-rows x 128)
-  //   encoder_1/simpleconv      ring over [B | C | W]: d1 is dead, u2 is written by its epilogue  5 stages x 8 KB (8 k-rows x 256)
-  static constexpr bool kDeep = S <= 8 && LYRA_B_DEEP_RINGS != 0 && kStg == kStages;
-  static constexpr int kStgR = kDeep ? 7 : kStg, kKcR = kDeep ? 8 : 16;
-  static constexpr int kStgD = kDeep ? 5 : kStg;
+  static constexpr int kI8Pd = 4;                         // k-steps of int8 weight fragments in flight from L2
   static constexpr int kI = kW + kWBytes;
   static constexpr int kSmemBytes = kI + 3 * S * 4 + 16;
-  static constexpr int kRingR = kDeep ? kRC : kW, kRingD = kDeep ? kRB : kW;
-  static_assert(kRingR + kStgR * kKcR * 128 * 4 <= kW + kWBytes && kRingD + kStgD * 8 * 256 * 4 <= kW + kWBytes, "borrowed rings end with region W");
-  static_assert(kRingR % 16 == 0 && kRingD % 16 == 0, "bulk-copy alignment");
 };
 
-template <int S>
-__global__ void __launch_bounds__(EncB<S>::NT, EncB<S>::kMinBlocks)
+__global__ void __launch_bounds__(EncB::NT, EncB::kMinBlocks)
 EncoderKernelB(const uint8_t* __restrict__ blob, EncoderParams P, TileIo io, const float* __restrict__ mid,
                float* __restrict__ state, int* __restrict__ n18g, float* __restrict__ features) {
-  using L = EncB<S>;
-  constexpr int NT = L::NT;
-  constexpr int TM = L::TM;
+  using L = EncB;
+  constexpr int S = L::S, NT = L::NT;
+  constexpr int TM = L::TM, TN = L::TN;
   unsigned char* smem = LYRA_DYN_SMEM();
   constexpr int LQ2 = L::LQ2, LQA = L::LQA, LQB = L::LQB;
   float* u1 = reinterpret_cast<float*>(smem + L::kRA);
@@ -472,10 +430,8 @@ EncoderKernelB(const uint8_t* __restrict__ blob, EncoderParams P, TileIo io, con
   uint32_t* stw = reinterpret_cast<uint32_t*>(state) + (size_t)tile * EncStateB::kUnits * S;
   float* st = reinterpret_cast<float*>(stw);
   const int tid = (int)threadIdx.x;
-  PrefetchTileState<LYRA_PREFETCH_STATE>(st, EncStateB::kUnits * S * 4);
-  float* ring_r = reinterpret_cast<float*>(smem + L::kRingR);       // encoder_1's ring
-  float* ring_d = reinterpret_cast<float*>(smem + L::kRingD);       // encoder_1/simpleconv's ring
-  IssuePrologue<NT>(ring_r, NextF32(BlobPtr<float>(blob, P.r1[0].pw1.w), L::kKcR, 128, 128, nullptr, L::kStgR));
+  PrefetchTileState(st, EncStateB::kUnits * S * 4);
+  IssuePrologue<NT>(wbuf, NextF32(BlobPtr<float>(blob, P.r1[0].pw1.w), 16, 128, 128, nullptr, L::kStg));
   int ph = 0;
   LYRA_PHASE(1, ph);
 
@@ -491,9 +447,9 @@ EncoderKernelB(const uint8_t* __restrict__ blob, EncoderParams P, TileIo io, con
   // ---- encoder_1: three residual units @128 (second 1x1 has 2 groups)
   LYRA_PHASE(1, ph);
   static_assert(EncStateB::kRing1 == EncStateB::kRing0 + 128 * 2 && EncStateB::kRing2 == EncStateB::kRing1 + 128 * 6, "ring blocks back to back");
-  ResUnitsF32x3<S, NT, TM, LYRA_BC_TN, LYRA_BC_TN, L::WM4, L::kKcR, 128, 4, false, 4 * S, 1, 1, L::kStgR>(
-      blob, P.r1, u1, L::LD1, 2, d1, 2, st + (size_t)EncStateB::kRing0 * S, n18, active, ring_r,
-      NextF32(BlobPtr<float>(blob, P.down1.w), 8, 256, 256, ring_d, L::kStgD), 1, ph);
+  ResUnitsF32x3<S, NT, TM, TN, TN, L::WM4, 16, 128, 4, false, 4 * S, 1, 1, L::kStg>(
+      blob, P.r1, u1, L::LD1, 2, d1, 2, st + (size_t)EncStateB::kRing0 * S, n18, active, wbuf,
+      NextF32(BlobPtr<float>(blob, P.down1.w), 8, 256, 256, wbuf, L::kStg), 1, ph);
   for (int i = tid; i < 128 * 2 * S; i += NT) {
     const int c = i / (2 * S), r = i % (2 * S);
     if (active[r % S]) st[EncStateB::kDown1 * S + i] = u1[(size_t)c * L::LD1 + 4 * S + r];
@@ -502,11 +458,11 @@ EncoderKernelB(const uint8_t* __restrict__ blob, EncoderParams P, TileIo io, con
   LYRA_PHASE(1, ph);
   {
     const float* b = BlobPtr<float>(blob, P.down1.bias);
-    GemmF32Tap<S, NT, TM, LYRA_BC_TN, 8, L::WM2, false, L::kStgD>(u1, L::LD1, 0, 2, 4, 64, 2, 2, 256, BlobPtr<float>(blob, P.down1.w), ring_d, true,
+    GemmF32Tap<S, NT, TM, TN, 8, L::WM2, false, L::kStg>(u1, L::LD1, 0, 2, 4, 64, 2, 2, 256, BlobPtr<float>(blob, P.down1.w), wbuf, true,
       NextF32(BlobPtr<float>(blob, P.m_pw1.w), 8, 256, 256, wbuf, L::kStg),
-      [&](int t, int s0, int n0, float (&acc)[TM][LYRA_BC_TN]) {
+      [&](int t, int s0, int n0, float (&acc)[TM][TN]) {
 #pragma unroll
-        for (int j = 0; j < LYRA_BC_TN; ++j) {
+        for (int j = 0; j < TN; ++j) {
           float* o = u2 + (size_t)(n0 + j) * 2 * S + t * S + s0;
 #pragma unroll
           for (int i = 0; i < TM; ++i) o[i] = __fadd_rn(acc[i][j], b[n0 + j]);
@@ -527,17 +483,17 @@ EncoderKernelB(const uint8_t* __restrict__ blob, EncoderParams P, TileIo io, con
     const float* b = BlobPtr<float>(blob, P.m_pw1.bias);
     const int8_t* lut = BlobPtr<int8_t>(blob, P.m_lr1.lut);
     const QuantP q1 = P.m_q1;
-    GemmF32Tap<S, NT, TM, LYRA_BC_TN, 8, L::WM2, false, L::kStg>(d2, LD2, 0, 1, 1, 256, 1, 2, 256, BlobPtr<float>(blob, P.m_pw1.w), wbuf, true,
+    static_assert(TN == 4, "the epilogue packs one word of four channels per (row, stream)");
+    GemmF32Tap<S, NT, TM, TN, 8, L::WM2, false, L::kStg>(d2, LD2, 0, 1, 1, 256, 1, 2, 256, BlobPtr<float>(blob, P.m_pw1.w), wbuf, true,
       NoNext(),
-      [&](int t, int s0, int n0, float (&acc)[TM][LYRA_BC_TN]) {
+      [&](int t, int s0, int n0, float (&acc)[TM][TN]) {
 #pragma unroll
         for (int i = 0; i < TM; ++i) {
-          int q[LYRA_BC_TN];
+          int q[TN];
 #pragma unroll
-          for (int j = 0; j < LYRA_BC_TN; ++j) q[j] = lut[QuantizeF32(__fadd_rn(acc[i][j], b[n0 + j]), q1.scale, q1.zp) + 128];
-          uint32_t* word = hq + (size_t)(n0 / 4) * LQ2 + t * S + s0 + i;       // channels 4k .. 4k+3 of one (row, stream), byte j = channel 4k + j
-          if constexpr (LYRA_BC_TN == 4) *word = PackI8x4(q[0], q[1], q[2], q[3]);
-          else reinterpret_cast<uint16_t*>(word)[(n0 % 4) / 2] = (uint16_t)((q[0] & 0xff) | ((q[1] & 0xff) << 8));
+          for (int j = 0; j < TN; ++j) q[j] = lut[QuantizeF32(__fadd_rn(acc[i][j], b[n0 + j]), q1.scale, q1.zp) + 128];
+          // channels 4k .. 4k+3 of one (row, stream), byte j = channel 4k + j
+          hq[(size_t)(n0 / 4) * LQ2 + t * S + s0 + i] = PackI8x4(q[0], q[1], q[2], q[3]);
         }
       });
   }
@@ -548,7 +504,7 @@ EncoderKernelB(const uint8_t* __restrict__ blob, EncoderParams P, TileIo io, con
     const int8_t* lut = BlobPtr<int8_t>(blob, P.m_lr2.lut);
     const QuantP dq = P.m_dq, q2 = P.m_q2;
     const int out_zp = P.m_pw2.out_zp;
-    GemmI8Mma<S, NT, (S >= 16 ? 8 : 4), L::kI8Pd>(hq, LQ2, 0, 1, 1, 64, 4, 2, 256, BlobPtr<uint2>(blob, P.m_pw2.w),
+    GemmI8Mma<S, NT, 4, L::kI8Pd>(hq, LQ2, 0, 1, 1, 64, 4, 2, 256, BlobPtr<uint2>(blob, P.m_pw2.w),
       [&](int t, int s, int n0, int (&acc)[1][4]) {
         const RequantP4 rq = LoadRequant4(bias, mult, shift, n0);
         int r[4], a[4];
@@ -625,12 +581,15 @@ EncoderKernelB(const uint8_t* __restrict__ blob, EncoderParams P, TileIo io, con
 // ================================================================================================
 //                                        DECODER  C
 // ================================================================================================
-template <int S, bool TC = false>
+template <bool TC = false>
 struct DecC {
+  static constexpr int S = kTileStreams;
   static constexpr int NT = 256;
-  static constexpr int kMinBlocks = S <= 8 ? LYRA_C_MIN_BLOCKS : 1;
-  static constexpr int kI8Pd = S <= 8 ? LYRA_C_I8_PD : LYRA_I8_PD;    // prefetch depth of the four-n-tile int8 GEMMs (the eight-n-tile upsamplers keep LYRA_I8_PD)
+  static constexpr int kMinBlocks = 3;                    // resident blocks per SM (59 KB of shared memory each)
+  static constexpr int kI8Pd = 2;                         // prefetch depth of the four-n-tile int8 GEMMs (the eight-n-tile upsamplers
+                                                          // take GemmI8Mma's default)
   static constexpr int TM = 8;                            // streams per fp32 thread tile (8 x 4 tiles: fewer smem wavefronts per FMA)
+  static constexpr int TN = 4;                            // output channels per fp32 thread tile (decoder_1)
   static constexpr int WM4 = 4 * S / TM >= 4 ? 4 : 4 * S / TM;   // m-groups per warp for T = 4 / 2 / 1 row layers
   static constexpr int WM2 = 2 * S / TM >= 4 ? 4 : 2 * S / TM;
   static constexpr int WM1 = 1 * S / TM >= 4 ? 4 : 1 * S / TM;
@@ -639,12 +598,11 @@ struct DecC {
   //   region 1: F f32 [64][3S] + xq words [128][LQB]  ->  aq words [64][LQA]  ->  d1 f32 [128][4S]
   //   region 2: u f32 [256][2S]  ->  u1 f32 [128][4S]
   //   region W: fp32 weight ring (bottleneck_2, decoder_1)  <->  hq, dq8, resq words [64][LQ2] each (int8 phases)
-  static constexpr int kMax(int a, int b) { return a > b ? a : b; }
   static constexpr int kF = 0;
   static constexpr int kXq = kF + 64 * 3 * S * 4;
   // tensor-core mode: d1 is an MMA A operand (padded stride); decoder_1 warp tiles: 2 m-tiles x RWN n-tiles
   static constexpr int LD1 = TC ? PadLd(4 * S) : 4 * S;
-  static constexpr int RWM = 2, RWN = S >= 16 ? 4 : 2;
+  static constexpr int RWM = 2, RWN = 2;
   static_assert(!TC || ((4 * S + 31) / 32) * (16 / RWN) <= NT / 32, "decoder_1: one warp tile per warp");
   static constexpr int kR1Bytes = kMax(kMax(64 * 3 * S * 4 + 128 * LQB * 4, 64 * LQA * 4), 128 * LD1 * 4);
   static constexpr int kU = kF + kR1Bytes;
@@ -654,14 +612,14 @@ struct DecC {
   static constexpr int kSmemBytes = kI + 3 * S * 4 + 16;
 };
 
-template <int S, bool TC>
-__global__ void __launch_bounds__(DecC<S, TC>::NT, DecC<S, TC>::kMinBlocks)
+template <bool TC>
+__global__ void __launch_bounds__(DecC<TC>::NT, DecC<TC>::kMinBlocks)
 DecoderKernelC(const uint8_t* __restrict__ blob, DecoderParams P, TileIo io,
                const float* __restrict__ features, float* __restrict__ state, int* __restrict__ n18g,
                float* __restrict__ mid) {
-  using L = DecC<S, TC>;
-  constexpr int NT = L::NT;
-  constexpr int TM = L::TM;
+  using L = DecC<TC>;
+  constexpr int S = L::S, NT = L::NT;
+  constexpr int TM = L::TM, TN = L::TN;
   unsigned char* smem = LYRA_DYN_SMEM();
   float* F = reinterpret_cast<float*>(smem + L::kF);
   uint32_t* xq = reinterpret_cast<uint32_t*>(smem + L::kXq);
@@ -684,7 +642,7 @@ DecoderKernelC(const uint8_t* __restrict__ blob, DecoderParams P, TileIo io,
   uint32_t* stw = reinterpret_cast<uint32_t*>(state) + (size_t)tile * DecStateC::kUnits * S;
   float* st = reinterpret_cast<float*>(stw);
   const int tid = (int)threadIdx.x;
-  PrefetchTileState<LYRA_PREFETCH_STATE>(st, DecStateC::kUnits * S * 4);
+  PrefetchTileState(st, DecStateC::kUnits * S * 4);
   constexpr int LD2 = 2 * S;
   const UpI8& up0 = P.up0;
   const UpI8& up1 = P.up1;
@@ -775,7 +733,7 @@ DecoderKernelC(const uint8_t* __restrict__ blob, DecoderParams P, TileIo io,
     const int* shift = BlobPtr<int>(blob, P.m_pw1.shift);
     const int8_t* lut = BlobPtr<int8_t>(blob, P.m_lr1.lut);
     const int out_zp = P.m_pw1.out_zp;
-    GemmI8Mma<S, NT, (S >= 16 ? 8 : 4), L::kI8Pd>(dq8, LQ2, 0, 1, 1, 256, 1, 2, 256, BlobPtr<uint2>(blob, P.m_pw1.w),
+    GemmI8Mma<S, NT, 4, L::kI8Pd>(dq8, LQ2, 0, 1, 1, 256, 1, 2, 256, BlobPtr<uint2>(blob, P.m_pw1.w),
       [&](int t, int s, int n0, int (&acc)[1][4]) {
         const RequantP4 rq = LoadRequant4(bias, mult, shift, n0);
         int q[4];
@@ -791,7 +749,7 @@ DecoderKernelC(const uint8_t* __restrict__ blob, DecoderParams P, TileIo io,
     const int8_t* lut = BlobPtr<int8_t>(blob, P.m_lr2.lut);
     const QuantP dq = P.m_dq, q2 = P.m_q2;
     const int out_zp = P.m_pw2.out_zp;
-    GemmI8Mma<S, NT, (S >= 16 ? 8 : 4), L::kI8Pd>(hq, LQ2, 0, 1, 1, 64, 4, 2, 256, BlobPtr<uint2>(blob, P.m_pw2.w),
+    GemmI8Mma<S, NT, 4, L::kI8Pd>(hq, LQ2, 0, 1, 1, 64, 4, 2, 256, BlobPtr<uint2>(blob, P.m_pw2.w),
       [&](int t, int s, int n0, int (&acc)[1][4]) {
         const RequantP4 rq = LoadRequant4(bias, mult, shift, n0);
         int r[4], a[4];
@@ -848,7 +806,7 @@ DecoderKernelC(const uint8_t* __restrict__ blob, DecoderParams P, TileIo io,
   // ---- decoder_1: three fp32 residual units @128
   LYRA_PHASE(2, ph);
   static_assert(DecStateC::kRing1 == DecStateC::kRing0 + 128 * 2 && DecStateC::kRing2 == DecStateC::kRing1 + 128 * 6, "ring blocks back to back");
-  ResUnitsF32x3<S, NT, TM, LYRA_BC_TN, LYRA_BC_TN, L::WM4, 16, 128, 4, TC, L::LD1, L::RWM, L::RWN>(
+  ResUnitsF32x3<S, NT, TM, TN, TN, L::WM4, 16, 128, 4, TC, L::LD1, L::RWM, L::RWN>(
       blob, P.r1, u1, 4 * S, 0, d1, 2, st + (size_t)DecStateC::kRing0 * S, n18, active, wbuf, NoNext(), 2, ph);
   {
     float* out = mid + (size_t)tile * 128 * 4 * S;
@@ -861,41 +819,36 @@ DecoderKernelC(const uint8_t* __restrict__ blob, DecoderParams P, TileIo io,
 // ================================================================================================
 //                                        DECODER  D
 // ================================================================================================
-template <int S, bool TC = false>
+// The exact decoder mode's kernel D (fp32 FMA chains, bit-exact with the oracle); the tensor mode runs DecoderKernelDW
+// (net_kernels_wgmma.cuh) instead.
 struct DecD {
+  static constexpr int S = kTileStreams;
   static constexpr int NT = 320;
-  static constexpr int TN = S >= 16 ? 8 : 4;
-  static constexpr int kMinBlocks = S <= 8 ? 2 : 1;
-  static constexpr int TNU = S >= 16 ? 10 : 5;            // decoder_2/simple column tile (320 columns)
-  static constexpr int TNL = S >= 16 ? 4 : 2;             // last_layer column tile (16 columns)
-  static constexpr int WML = S >= 16 ? 8 : 4;
-  static constexpr int WMU = S >= 16 ? 2 : 1;
+  static constexpr int TN = 4;
+  static constexpr int kMinBlocks = 2;
+  static constexpr int TNU = 5;                           // decoder_2/simple column tile (320 columns)
+  static constexpr int TNL = 2;                           // last_layer column tile (16 columns)
+  static constexpr int WML = 4;
+  static constexpr int WMU = 1;
   static constexpr int KCU = 8;                           // its ring starts right behind X inside d and runs into the regular ring
-  // u: 3 zero rows + 20 + 3 zero rows.  Tensor-core mode pads the strides of the MMA A operands (u, d, X) and
-  // needs no weight ring (weights go from L2 straight into fragments).
-  static constexpr int LDU = TC ? PadLd(26 * S) : 26 * S, LDD = TC ? PadLd(20 * S) : 20 * S, LDX = TC ? PadLd(6 * S) : 6 * S;
+  static constexpr int LDU = 26 * S, LDD = 20 * S, LDX = 6 * S;   // u: 3 zero rows + 20 + 3 zero rows
   static constexpr int kU = 0;
   static constexpr int kD = kU + 64 * LDU * 4;              // d f32 [64][LDD]; aliases X f32 [128][LDX] and the PCM staging
   static constexpr int kW = kD + 64 * LDD * 4;
-  static constexpr int kWBytes = TC ? 0 : kStages * 16 * 64 * 4 + 2048;   // regular ring (64-channel layers) + slack for the decoder_2/simple ring
+  static constexpr int kWBytes = kStages * 16 * 64 * 4 + 2048;   // regular ring (64-channel layers) + slack for the decoder_2/simple ring
   static constexpr int kSl = kW + kWBytes;                  // carried tail of last_layer [48][S]
-  static_assert(TC || 128 * 6 * S * 4 + kStages * KCU * 320 * 4 <= 64 * LDD * 4 + kWBytes, "decoder_2/simple ring must fit behind X");
+  static_assert(128 * 6 * S * 4 + kStages * KCU * 320 * 4 <= 64 * LDD * 4 + kWBytes, "decoder_2/simple ring must fit behind X");
   static constexpr int kI = kSl + 48 * S * 4;
   static constexpr int kSmemBytes = kI + 3 * S * 4 + 16;
   static_assert(128 * LDX <= 64 * LDD, "X must fit in d");
   static_assert(S * 320 * 2 <= 64 * LDD * 4, "PCM staging must fit in d");
-  // tensor-core warp tiles: decoder_2 res-units RWM x RWN (one per warp), decoder_2/simple UWM x 2, last_layer 1 x 1
-  static constexpr int RWM = S >= 16 ? 4 : 2, RWN = NT >= 320 ? 4 : 8;
-  static constexpr int UWM = (5 * S + 15) / 16;
-  static_assert(!TC || ((20 * S / 16 + RWM - 1) / RWM) * (8 / RWN) <= NT / 32, "decoder_2: one warp tile per warp");
 };
 
-template <int S, bool TC>
-__global__ void __launch_bounds__(DecD<S, TC>::NT, DecD<S, TC>::kMinBlocks)
+__global__ void __launch_bounds__(DecD::NT, DecD::kMinBlocks)
 DecoderKernelD(const uint8_t* __restrict__ blob, DecoderParams P, TileIo io, const float* __restrict__ mid,
                float* __restrict__ state, int* __restrict__ n18g, int16_t* __restrict__ pcm) {
-  using L = DecD<S, TC>;
-  constexpr int NT = L::NT;
+  using L = DecD;
+  constexpr int S = L::S, NT = L::NT;
   unsigned char* smem = LYRA_DYN_SMEM();
   float* u = reinterpret_cast<float*>(smem + L::kU);
   float* d = reinterpret_cast<float*>(smem + L::kD);
@@ -911,10 +864,10 @@ DecoderKernelD(const uint8_t* __restrict__ blob, DecoderParams P, TileIo io, con
   if (n18[S] == kTileIdle) return;
   float* st = state + (size_t)tile * DecStateD::kUnits * S;
   const int tid = (int)threadIdx.x;
-  PrefetchTileState<LYRA_PREFETCH_STATE>(st, DecStateD::kUnits * S * 4);
+  PrefetchTileState(st, DecStateD::kUnits * S * 4);
   constexpr int LDX = L::LDX;
   float* wbuf_up2 = X + 128 * LDX;       // free tail of d + the regular ring
-  if (!TC) IssuePrologue<NT>(wbuf_up2, NextF32(BlobPtr<float>(blob, P.up2.w), L::KCU, 320, 256));
+  IssuePrologue<NT>(wbuf_up2, NextF32(BlobPtr<float>(blob, P.up2.w), L::KCU, 320, 256));
   int ph = 0;
   LYRA_PHASE(3, ph);
 
@@ -957,16 +910,13 @@ DecoderKernelD(const uint8_t* __restrict__ blob, DecoderParams P, TileIo io, con
         }
       }
     };
-    if constexpr (TC)
-      GemmTf32Mma<S, NT, L::UWM, 2, false>(X, LDX, 0, 1, 2, 128, 1, 5, 320, BlobPtr<float2>(blob, P.up2.wf), epi_up);
-    else
-      GemmF32Tap<S, NT, 8, L::TNU, L::KCU, L::WMU, false>(X, LDX, 0, 1, 2, 128, 1, 5, 320, BlobPtr<float>(blob, P.up2.w), wbuf_up2, true,
-                                                          NextF32(BlobPtr<float>(blob, P.r2[0].pw1.w), 16, 64, 64, wbuf), epi_up);
+    GemmF32Tap<S, NT, 8, L::TNU, L::KCU, L::WMU, false>(X, LDX, 0, 1, 2, 128, 1, 5, 320, BlobPtr<float>(blob, P.up2.w), wbuf_up2, true,
+                                                        NextF32(BlobPtr<float>(blob, P.r2[0].pw1.w), 16, 64, 64, wbuf), epi_up);
   }
   // ---- decoder_2: three residual units @64, T = 20
   LYRA_PHASE(3, ph);
   static_assert(DecStateD::kRing1 == DecStateD::kRing0 + 64 * 2 && DecStateD::kRing2 == DecStateD::kRing1 + 64 * 6, "ring blocks back to back");
-  ResUnitsF32x3<S, NT, 8, L::TN, L::TN, 4, 16, 64, 20, TC, L::LDD, L::RWM, L::RWN>(blob, P.r2, u, L::LDU, 3, d, 1, st + (size_t)DecStateD::kRing0 * S, n18, active, wbuf,
+  ResUnitsF32x3<S, NT, 8, L::TN, L::TN, 4, 16, 64, 20>(blob, P.r2, u, L::LDU, 3, d, 1, st + (size_t)DecStateD::kRing0 * S, n18, active, wbuf,
                                                        NextF32(BlobPtr<float>(blob, P.last.w), 16, 16, 256), 3, ph);
   // ---- last_layer: TRANSPOSE_CONV K = 64, stride 16, 64 -> 1 ; T 20 -> 320 (+48 tail) ; float -> int16
   LYRA_PHASE(3, ph);
@@ -994,10 +944,7 @@ DecoderKernelD(const uint8_t* __restrict__ blob, DecoderParams P, TileIo io, con
         }
       }
     };
-    if constexpr (TC)
-      GemmTf32Mma<S, NT, 1, 1, false>(u, L::LDU, 0, 1, 4, 64, 1, 23, 16, BlobPtr<float2>(blob, P.last.wf), epi_last);
-    else
-      GemmF32Tap<S, NT, 8, L::TNL, 16, L::WML, false>(u, L::LDU, 0, 1, 4, 64, 1, 23, 16, BlobPtr<float>(blob, P.last.w), wbuf, true, NoNext(), epi_last);
+    GemmF32Tap<S, NT, 8, L::TNL, 16, L::WML, false>(u, L::LDU, 0, 1, 4, 64, 1, 23, 16, BlobPtr<float>(blob, P.last.w), wbuf, true, NoNext(), epi_last);
     for (int i = tid; i < S * 320; i += NT) {
       const int s = i / 320;
       if (active[s]) pcm[(size_t)slot[s] * 320 + (i % 320)] = stage[i];

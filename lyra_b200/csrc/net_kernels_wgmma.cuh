@@ -36,7 +36,8 @@
 namespace lyra_b200 {
 
 struct DecDW {
-  static constexpr int S = 8;
+  static constexpr int S = kTileStreams;
+  static_assert(S == 8, "the row warps map lane / 4 to the tile's stream");
   static constexpr int kRowWgs = 3, kRowThreads = kRowWgs * 128;
   static constexpr int kTmaWarp = kRowThreads / 32;
   static constexpr int NT = kRowThreads + 32;
@@ -133,7 +134,7 @@ DecoderKernelDW(const uint8_t* __restrict__ blob, DecoderParams P, TileIo io, co
   if (n18[S] == kTileIdle) return;
   float* st = state + (size_t)tile * DecStateD::kUnits * S;
   const uint8_t* chunks = blob + P.du_chunks;
-  PrefetchTileState<LYRA_PREFETCH_STATE>(st, DecStateD::kUnits * S * 4);      // unit 2 reads its ring block from global memory
+  PrefetchTileState(st, DecStateD::kUnits * S * 4);                          // unit 2 reads its ring block from global memory
 
   // ================================================= TMA producer =================================================
   if (warp == L::kTmaWarp) {

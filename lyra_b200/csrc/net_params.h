@@ -17,8 +17,8 @@
 namespace lyra_b200 {
 
 // fp32 GEMM-shaped convolution: weights [Ktot][N] k-major (k = tap*CinG + ci), bias [N]
-// wf: the same [K][N] matrix in mma.sync m16n8k8 B-fragment order [K/8][N/8][32 lanes] x float2 (decoder layers only;
-// 0 = not packed) for the decoder's tensor-core mode
+// wf: the same [K][N] matrix in mma.sync m16n8k8 B-fragment order [K/8][N/8][32 lanes] x float2, which GemmTf32Mma reads in
+// kernel C's tensor mode; only decoder_1's residual-unit 1x1 convolutions (DecoderParams::r1[*].pw1 / pw2) carry it (0 elsewhere)
 struct GemmF32 { uint32_t w, bias, wf; };
 // int8 convolution: weights in mma.sync m16n8k32 B-fragment order [Ktot/32][N/8][32 lanes][2 words]
 // (k = tap*CinG + ci), bias folded with the input zero point (bias + (-zp_in) * sum(w)), per-channel Q31

@@ -77,12 +77,6 @@ def test_emu_priority_switch(emu_api, oracle):
     pc.run_priority_switch(_capi.Context, emu_api, oracle, n=2, frames=3)
 
 
-def test_emu_sixteen_stream_tiles(emu_api, oracle, monkeypatch):
-    monkeypatch.setenv("LYRA_B200_TILE_STREAMS", "16")
-    pc.run_codec_parity(_capi.Context, emu_api, oracle, max_streams=32, stream_ids=[3, 17], frames=3, bits=64)
-    pc.run_codec_parity(_capi.Context, emu_api, oracle, max_streams=16, stream_ids=[5], frames=2, bits=64, decoder_mode="tensor")
-
-
 def test_emu_role_contexts(emu_api, oracle):
     pc.run_role_contexts(_capi.Context, emu_api, oracle, _capi.LyraB200Error, frames=2)
 

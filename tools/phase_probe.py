@@ -1,6 +1,8 @@
 #!/usr/bin/env python3
 """Dev tool (GPU): per-phase clock64() breakdown of the four conv-net kernels using the -DLYRA_PHASE_PROF build
-(devtools_build/liblyra_b200_phase.so, built by hand with nvcc ... -DLYRA_PHASE_PROF)."""
+(devtools_build/liblyra_b200_phase.so: tools/build_variant.sh phase -DLYRA_PHASE_PROF).
+
+usage: tools/phase_probe.py [streams] [split] [exact|tensor]    (decoder mode, default exact)"""
 import ctypes as C
 import os
 import sys
@@ -30,6 +32,9 @@ def main():
     ctx = _capi.Context(n, capi=api)
     if len(sys.argv) > 2:
         ctx.set_split(int(sys.argv[2]))          # 1 = one launch per kernel for the whole batch (no concurrent sub-batches)
+    du = len(sys.argv) > 3 and sys.argv[3] == "tensor"
+    if du:
+        ctx.set_decoder_mode("tensor")           # kernel 3 is then DecoderKernelDW
     buf = np.zeros((4, 1024, 48), dtype=np.int64)
     api.lib.lyra_b200_debug_phases(ctx.h, buf.ctypes.data_as(C.c_void_p))      # arms the buffer
     rng = np.random.default_rng(0)
@@ -39,7 +44,6 @@ def main():
         ctx.decode(pk, 64)
     api.lib.lyra_b200_debug_phases(ctx.h, buf.ctypes.data_as(C.c_void_p))
     nblk = min(1024, n // ctx.tile_streams)
-    du = os.environ.get("LYRA_B200_DECODER_MODE") == "tensor"
     if du:
         NAMES[3] = ["loads+X", "up2 split (weight stream)", "up2 mma tail", "up2 epi"] + sum([["u%d ring wait" % i, "u%d dw" % i, "u%d ring upd" % i, "u%d pw1 mma" % i, "u%d epi1" % i,
                                                           "u%d pw2 mma" % i, "u%d epi2" % i] for i in range(3)], []) + ["last (4 taps)", "last epi+store"]

@@ -14,13 +14,14 @@ import sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 LIB = os.path.join(ROOT, "lyra_b200", "liblyra_b200.so")
 
-# headline instantiations (8-stream tiles; DecoderKernelC<8,true> feeds DecoderKernelDW in the tensor mode)
+# mangled-name patterns (DecoderKernelC<true> feeds DecoderKernelDW in the tensor mode, DecoderKernelC<false> DecoderKernelD in the
+# exact mode)
 KERNELS = {
-    "EncoderKernelA": r"EncoderKernelAILi8E",
-    "EncoderKernelB": r"EncoderKernelBILi8E",
-    "DecoderKernelC_tensor": r"DecoderKernelCILi8ELb1E",
-    "DecoderKernelC_exact": r"DecoderKernelCILi8ELb0E",
-    "DecoderKernelD_exact": r"DecoderKernelDILi8ELb0E",
+    "EncoderKernelA": r"EncoderKernelAE",
+    "EncoderKernelB": r"EncoderKernelBE",
+    "DecoderKernelC_tensor": r"DecoderKernelCILb1E",
+    "DecoderKernelC_exact": r"DecoderKernelCILb0E",
+    "DecoderKernelD_exact": r"DecoderKernelDE",
     "DecoderKernelDW": r"DecoderKernelDWE",
     "RvqEncodeKernel": r"RvqEncodeKernelE",
     "RvqDecodeKernel": r"RvqDecodeKernelE",
