@@ -167,7 +167,10 @@ int lyra_b200_resample(lyra_b200_ctx* ctx, int to_internal, const int32_t* strea
 
 /* ---- device-resident variants (pointers are CUDA device pointers; asynchronous on the context's
  *      stream; streams 0..n-1).  Used by bench.py for the HBM-resident `value` measurement and by
- *      callers that keep audio on the GPU. ---------------------------------------------------------- */
+ *      callers that keep audio on the GPU.  A call does not wait for the work it queues or for earlier
+ *      work on the installed stream, reads its inputs and writes its outputs only in stream order on the installed stream, and
+ *      touches no row outside [0, n) of the caller's buffers (so several contexts may work on slices of one
+ *      buffer).  Role checks are those of the host-buffer twins: noise_update_device works in any context. ---- */
 int lyra_b200_set_stream(lyra_b200_ctx* ctx, void* cuda_stream); /* NULL restores the context's own stream */
 int lyra_b200_encode_device(lyra_b200_ctx* ctx, int n, const int16_t* d_pcm, int num_bits, uint8_t* d_packets);
 int lyra_b200_decode_device(lyra_b200_ctx* ctx, int n, const uint8_t* d_packets, const uint8_t* d_received,

@@ -1089,7 +1089,7 @@ int lyra_b200_noise_update_device(lyra_b200_ctx* ctx, int n, const int16_t* d_pc
                                   uint8_t* d_is_noise, float* d_noise_estimate) {
   if (!ctx || !d_pcm) return LYRA_B200_EINVAL;
   if (cudaSetDevice(ctx->device) != cudaSuccess) { ctx->err = "cudaSetDevice failed"; return LYRA_B200_ENODEV; }   // the current device is per host thread
-  if (!RoleOk(ctx, LYRA_B200_ROLE_DECODER)) return LYRA_B200_EINVAL;
+  // no role check: the estimators are self-contained and allocated in every context, as for lyra_b200_noise_update
   if (n <= 0 || n > ctx->max_streams) { ctx->err = "stream count out of range"; return LYRA_B200_EINVAL; }
   return LaunchNoiseUpdate(ctx, ctx->stream, nullptr, 0, n, n, d_pcm, d_update_mask, d_is_noise, d_noise_estimate);
 }

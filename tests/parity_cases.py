@@ -229,9 +229,10 @@ def run_decode_track_noise_parity(Context, api, O, wav, *, n=3, frames=12, max_s
     ctx.close()
 
 
-def run_role_contexts(Context, api, O, LyraB200Error, *, frames=4, seed=9):
+def run_role_contexts(Context, api, O, LyraB200Error, mem, *, frames=4, seed=9):
     """lyra_b200_create_ex: an encoder-only and a decoder-only context together reproduce the oracle; calls of the missing
-    role are refused with EINVAL (the mirror of LyraEncoder / LyraDecoder being separate objects)."""
+    role are refused with EINVAL (the mirror of LyraEncoder / LyraDecoder being separate objects), the device-resident
+    variants included.  `mem` provides device buffers (HostMem / a torch-backed equivalent)."""
     n = 3
     enc = Context(8, capi=api, roles="encoder")
     dec = Context(8, capi=api, roles="decoder")
@@ -245,8 +246,16 @@ def run_role_contexts(Context, api, O, LyraB200Error, *, frames=4, seed=9):
             opkt, _, _ = codecs[k].encode(pcm[k], 120)
             opcm, _, _ = codecs[k].decode(opkt, 120)
             assert bytes(pk[k]) == opkt and np.array_equal(out[k], opcm), (f, k)
+    d_pcm, d_pk = mem.zeros((n, 320), np.int16), mem.zeros((n, 15), np.uint8)
+    d_flags, d_est = mem.zeros(n, np.uint8), mem.zeros((n, 160), np.float32)
+    mem.put(d_pcm, pcm)
+    p = mem.ptr
     for bad in (lambda: enc.decode(pk, 120), lambda: dec.encode(pcm, 120), lambda: enc.decode_plc(pk, 120),
-                lambda: dec.encode_dtx(pcm, 120), lambda: dec.extract_features(pcm)):
+                lambda: dec.encode_dtx(pcm, 120), lambda: dec.extract_features(pcm),
+                lambda: dec.encode_device(n, p(d_pcm), 120, p(d_pk)), lambda: enc.decode_device(n, p(d_pk), 0, 120, p(d_pcm)),
+                lambda: enc.decode_track_noise_device(n, p(d_pk), 0, 120, p(d_pcm)),
+                lambda: enc.decode_plc_device(n, p(d_pk), 0, 120, p(d_pcm)),
+                lambda: dec.encode_dtx_device(n, p(d_pcm), 120, p(d_pk), p(d_flags))):
         try:
             bad()
             raise AssertionError("a call of the missing role must fail")
@@ -254,6 +263,17 @@ def run_role_contexts(Context, api, O, LyraB200Error, *, frames=4, seed=9):
             assert e.code == -1
     assert enc.quantize(np.zeros((1, 64), dtype=np.float32), 64).shape == (1, 8)      # stateless calls work in any context
     assert enc.noise_update(pcm)[1].shape == (n, 160)                                  # ... and so do the self-contained estimators
+    # ... through the device-resident variant as well: the encoder-only context's second hop, against a fresh oracle estimator
+    # fed the same two hops
+    mem.put(d_pcm, pcm)
+    enc.set_stream(mem.stream)
+    enc.noise_update_device(n, p(d_pcm), 0, p(d_flags), p(d_est))
+    enc.set_stream(None)
+    for k in range(n):
+        est = O.NoiseEstimator()
+        est.receive_samples(pcm[k])
+        est.receive_samples(pcm[k])
+        assert mem.get(d_flags)[k] == int(est.is_noise) and np.array_equal(mem.get(d_est)[k], est.noise_estimate()), k
     enc.reset()
     dec.reset()
     enc.close()
@@ -419,3 +439,211 @@ def run_integration_other_rates(Context, api, O, *, rate, wav, bits=64, hops=60)
             worst = max(worst, O.log_spectral_distance(fi, fo))
     ctx.close()
     return worst
+
+
+# ---- the device-resident entry points (lyra_b200_*_device, lyra_b200_set_stream) ----
+
+class HostMem:
+    """Device buffers of the emulated library: cudaMalloc returns host memory there, so numpy arrays stand in for device
+    memory and pointers are their addresses.  The GPU tier passes an equivalent built on torch CUDA tensors."""
+    stream = None           # the emulator has no streams to install
+
+    def zeros(self, shape, dtype):
+        return np.zeros(shape, dtype)
+
+    def ptr(self, buf):
+        return buf.ctypes.data
+
+    def put(self, buf, a):
+        buf[...] = a
+
+    def get(self, buf):
+        return np.array(buf)
+
+
+GUARD_ROWS = 3
+
+
+class Guarded:
+    """A caller buffer of n rows with GUARD_ROWS rows of a sentinel byte on each side: `ptr` is the address of row 0.  put()
+    rewrites the sentinels, get() checks that no call wrote outside rows [0, n).  fill() sets the n rows to the sentinel too,
+    so an output row that a call fails to write does not silently keep an earlier, correct value."""
+
+    def __init__(self, mem, n, row, dtype, sentinel):
+        self.mem, self.n = mem, n
+        self.shape = (n + 2 * GUARD_ROWS,) + tuple(row)
+        self.row_bytes = int(np.prod(row, dtype=np.int64)) * np.dtype(dtype).itemsize
+        self.sentinel = np.frombuffer(np.array([sentinel] * np.dtype(dtype).itemsize, np.uint8).tobytes(), dtype)[0]
+        self.dtype = dtype
+        self.buf = mem.zeros(self.shape, dtype)
+        self.fill()
+
+    @property
+    def ptr(self):
+        return self.mem.ptr(self.buf) + GUARD_ROWS * self.row_bytes
+
+    def put(self, a=None):
+        full = np.full(self.shape, self.sentinel, self.dtype)
+        if a is not None:
+            full[GUARD_ROWS:GUARD_ROWS + self.n] = a
+        self.mem.put(self.buf, full)
+
+    def fill(self):
+        self.put(None)
+
+    def get(self, what="buffer"):
+        a = self.mem.get(self.buf)
+        g = GUARD_ROWS
+        assert (a[:g] == self.sentinel).all() and (a[g + self.n:] == self.sentinel).all(), \
+            "a call wrote outside rows [0, %d) of the caller's %s" % (self.n, what)
+        return a[g:g + self.n]
+
+
+def _device_case_pcm(wav, n, f, frames):
+    """Hop f of the device-entry-point case: speech for streams k % 3 == 0, digital silence for the first half then speech for
+    k % 3 == 1, speech then silence for k % 3 == 2 (so DTX, the noise branch of the estimators and a restart from DTX all run)."""
+    pcm = np.stack([wav[(320 * (f + 13 * k + 20)) % (len(wav) - 320):][:320] for k in range(n)]).copy()
+    for k in range(n):
+        if (k % 3 == 1 and f < frames // 2) or (k % 3 == 2 and f >= frames // 2):
+            pcm[k] = 0
+    return pcm
+
+
+def run_device_parity(Context, api, O, mem, wav, *, n, frames, check, decoder_mode="exact", split=None, cng_seed=11, seed=3):
+    """Every *_device entry point against its host-buffer twin on a second context (all n streams), and a sample of streams
+    (`check`) against the oracle, hop by hop.  The device contexts run on mem.stream when there is one (lyra_b200_set_stream),
+    their inputs and outputs are caller buffers with guard rows (Guarded), outputs are pre-filled with a sentinel.
+    Covered: encode / decode with and without a received mask and with a bit-rate change between hops; decode_track_noise
+    (PCM, is_noise, the estimate read back at the end); noise_update with and without a mask, in an encoder-only context;
+    decode_plc with bursts long enough to reach comfort noise (PCM, flags, control state); encode_dtx over speech and silence
+    (empty-packet flags, zeroed bytes, the encoder state held on DTX hops).  n need not be a multiple of the tile size.
+    Bar: twins bit-exact in both decoder modes; oracle bit-exact, decoded PCM within TENSOR_PCM_TOL_LSB in the tensor mode."""
+    tol = TENSOR_PCM_TOL_LSB if decoder_mode == "tensor" else 0
+    exact = decoder_mode == "exact"
+    roles = dict(enc="encoder", dec="decoder", trk="decoder", plc="decoder", dtx="encoder", nz="encoder")
+    dev = {k: Context(n, capi=api, roles=r) for k, r in roles.items()}
+    host = {k: Context(n, capi=api, roles=r) for k, r in roles.items()}
+    for k in ("dec", "trk", "plc"):
+        dev[k].set_decoder_mode(decoder_mode)
+        host[k].set_decoder_mode(decoder_mode)
+    dev["plc"].set_cng_seed(cng_seed)
+    host["plc"].set_cng_seed(cng_seed)
+    for c in dev.values():
+        if split is not None:
+            c.set_split(split)
+        if mem.stream is not None:
+            c.set_stream(mem.stream)
+    G = lambda row, dtype, s: Guarded(mem, n, row, dtype, s)     # noqa: E731
+    d_pcm, d_zero = G((320,), np.int16, 0x3C), G((320,), np.int16, 0x3C)
+    d_rec, d_plc_rec, d_nz_mask = G((), np.uint8, 0xC3), G((), np.uint8, 0xC3), G((), np.uint8, 0xC3)
+    d_out, d_trk_out, d_plc_out = G((320,), np.int16, 0x5A), G((320,), np.int16, 0x5A), G((320,), np.int16, 0x5A)
+    d_trk_flags, d_cn, d_nz_flags, d_dtx_flags = (G((), np.uint8, 0xAA) for _ in range(4))
+    d_est = G((160,), np.float32, 0x7F)
+    d_zero.put(np.zeros((n, 320), np.int16))
+    codecs = {k: O.Codec(MODEL_DIR) for k in check}
+    trk_est = {k: O.NoiseEstimator() for k in check}
+    nz_est = {k: O.NoiseEstimator() for k in check}
+    plc_dec = {k: O.Decoder(MODEL_DIR, cng_seed=cng_seed + k) for k in check}
+    dtx_enc = {k: O.Encoder(MODEL_DIR, enable_dtx=True) for k in check}
+    rng = np.random.default_rng(seed)
+    burst = [(1 + k % 3, 8 if k % 2 == 0 else 2) for k in range(n)]      # (first lost hop, length) of each stream's outage
+    seen_dtx, seen_cn = set(), False
+    for f in range(frames):
+        bits = (64, 120, 184)[(f // 3) % 3]                               # the bit rate changes every third hop
+        P = (bits + 7) // 8
+        pcm = _device_case_pcm(wav, n, f, frames)
+        d_pcm.put(pcm)
+        # encode_device / decode_device (received mask on odd hops only: NULL = all received); the decoders read the packets
+        # where the encoder wrote them
+        d_pk, d_dtx_pk = G((P,), np.uint8, 0xA5), G((P,), np.uint8, 0xFF)
+        d_out.fill()
+        dev["enc"].encode_device(n, d_pcm.ptr, bits, d_pk.ptr)
+        rec = None
+        if f % 2:          # random, not periodic: a sub-batch that read another part's mask rows must see a different mask
+            rec = (rng.random(n) >= 0.25).astype(np.uint8)
+            d_rec.put(rec)
+        dev["dec"].decode_device(n, d_pk.ptr, d_rec.ptr if rec is not None else 0, bits, d_out.ptr)
+        pk = host["enc"].encode(pcm, bits)
+        out = host["dec"].decode(pk, bits, received=rec)
+        pk_rows = d_pk.get("packets")
+        assert np.array_equal(pk_rows, pk), "encode_device != encode, hop %d" % f
+        assert np.array_equal(d_out.get("PCM"), out), "decode_device != decode, hop %d" % f
+        # decode_track_noise_device (same packets and mask)
+        d_trk_out.fill()
+        d_trk_flags.fill()
+        dev["trk"].decode_track_noise_device(n, d_pk.ptr, d_rec.ptr if rec is not None else 0, bits, d_trk_out.ptr, d_trk_flags.ptr)
+        t_out, t_flags = host["trk"].decode_track_noise(pk, bits, received=rec)
+        assert np.array_equal(d_trk_out.get("PCM"), t_out), "decode_track_noise_device PCM != twin, hop %d" % f
+        assert np.array_equal(d_trk_flags.get("is_noise"), t_flags.astype(np.uint8)), "is_noise != twin, hop %d" % f
+        # noise_update_device in an encoder-only context (mask on even hops)
+        mask = (rng.random(n) < 0.8).astype(np.uint8) if f % 2 == 0 else None
+        if mask is not None:
+            d_nz_mask.put(mask)
+        d_nz_flags.fill()
+        d_est.fill()
+        dev["nz"].noise_update_device(n, d_pcm.ptr, d_nz_mask.ptr if mask is not None else 0, d_nz_flags.ptr, d_est.ptr)
+        nz_flags, nz_est_h = host["nz"].noise_update(pcm, update_mask=mask)
+        assert np.array_equal(d_nz_flags.get("is_noise"), nz_flags.astype(np.uint8)), "noise_update_device flags != twin, hop %d" % f
+        assert np.array_equal(d_est.get("estimate"), nz_est_h), "noise_update_device estimate != twin, hop %d" % f
+        # decode_plc_device: bursts of 8 lost hops (concealment -> fade -> comfort noise -> fade back) and of 2
+        plc_rec = np.array([0 if b0 <= f < b0 + bl else 1 for b0, bl in burst], dtype=np.uint8)
+        d_plc_rec.put(plc_rec)
+        d_plc_out.fill()
+        d_cn.fill()
+        dev["plc"].decode_plc_device(n, d_pk.ptr, d_plc_rec.ptr, bits, d_plc_out.ptr, d_cn.ptr)
+        p_out, p_cn = host["plc"].decode_plc(pk, bits, received=plc_rec)
+        assert np.array_equal(d_plc_out.get("PCM"), p_out), "decode_plc_device PCM != twin, hop %d" % f
+        assert np.array_equal(d_cn.get("flags"), p_cn.astype(np.uint8)), "decode_plc_device flags != twin, hop %d" % f
+        st = dev["plc"].plc_state(n)
+        assert np.array_equal(st, host["plc"].plc_state(n)), "control state != twin, hop %d" % f
+        seen_cn |= bool(p_cn.any())
+        # encode_dtx_device (its packet buffer starts as 0xFF bytes: the empty packets' zeros are written by the call)
+        d_dtx_flags.fill()
+        dev["dtx"].encode_dtx_device(n, d_pcm.ptr, bits, d_dtx_pk.ptr, d_dtx_flags.ptr)
+        x_pk, x_sizes = host["dtx"].encode_dtx(pcm, bits)
+        got_flags = d_dtx_flags.get("empty-packet flags")
+        got_pk = d_dtx_pk.get("packets")
+        assert np.array_equal(got_flags, (x_sizes == 0).astype(np.uint8)), "encode_dtx_device flags != twin, hop %d" % f
+        assert np.array_equal(got_pk, x_pk), "encode_dtx_device packets != twin, hop %d" % f
+        assert not got_pk[got_flags == 1].any(), "an empty packet's bytes must be zero"
+        seen_dtx |= set(int(x) for x in got_flags)
+        for k in check:
+            opkt, _, _ = codecs[k].encode(pcm[k], bits)
+            assert bytes(pk_rows[k]) == opkt, "packet != oracle, hop %d stream %d" % (f, k)
+            lost = rec is not None and rec[k] == 0
+            opcm, _, _ = codecs[k].decode(None if lost else opkt, bits)
+            for name, got in (("decode_device", out[k]), ("decode_track_noise_device", t_out[k])):
+                d = int(np.abs(got.astype(int) - opcm.astype(int)).max())
+                assert d <= tol, "%s PCM != oracle, hop %d stream %d: max |d| %d" % (name, f, k, d)
+            if exact:            # in the tensor mode the estimator is fed PCM that may differ by a few LSB: twins only
+                if not lost:
+                    trk_est[k].receive_samples(opcm)
+                assert bool(t_flags[k]) == trk_est[k].is_noise, "track is_noise != oracle, hop %d stream %d" % (f, k)
+            if mask is None or mask[k]:
+                nz_est[k].receive_samples(pcm[k])
+            assert bool(nz_flags[k]) == nz_est[k].is_noise and np.array_equal(nz_est_h[k], nz_est[k].noise_estimate()), \
+                "noise_update != oracle, hop %d stream %d" % (f, k)
+            if plc_rec[k]:
+                assert plc_dec[k].set_encoded_packet(opkt)
+            want = plc_dec[k].decode_samples(320)
+            d = int(np.abs(p_out[k].astype(int) - want.astype(int)).max())
+            assert d <= tol, "decode_plc PCM != oracle, hop %d stream %d: max |d| %d" % (f, k, d)
+            assert tuple(int(x) for x in st[k]) == plc_dec[k].state and bool(p_cn[k]) == plc_dec[k].is_comfort_noise(), (f, k)
+            want = dtx_enc[k].encode(pcm[k], bits)
+            assert x_sizes[k] == len(want) and bytes(x_pk[k][:x_sizes[k]]) == want, "encode_dtx != oracle, hop %d stream %d" % (f, k)
+        d_pcm.get("input PCM")                   # inputs are read only
+    assert seen_dtx == {0, 1}, "the case must produce both DTX and encoded hops"
+    assert seen_cn, "the case never reached comfort noise"
+    # the tracked estimates, read back through noise_update_device without feeding (mask all zero)
+    d_nz_mask.put(np.zeros(n, np.uint8))
+    d_est.fill()
+    d_trk_flags.fill()
+    dev["trk"].noise_update_device(n, d_zero.ptr, d_nz_mask.ptr, d_trk_flags.ptr, d_est.ptr)
+    h_flags, h_est = host["trk"].noise_update(np.zeros((n, 320), np.int16), update_mask=np.zeros(n, np.uint8))
+    est = d_est.get("estimate")
+    assert np.array_equal(est, h_est) and np.array_equal(d_trk_flags.get("is_noise"), h_flags.astype(np.uint8))
+    if exact:
+        for k in check:
+            assert np.array_equal(est[k], trk_est[k].noise_estimate()), "tracked estimate != oracle, stream %d" % k
+    for c in list(dev.values()) + list(host.values()):
+        c.close()

@@ -78,7 +78,12 @@ def test_emu_priority_switch(emu_api, oracle):
 
 
 def test_emu_role_contexts(emu_api, oracle):
-    pc.run_role_contexts(_capi.Context, emu_api, oracle, _capi.LyraB200Error, frames=2)
+    pc.run_role_contexts(_capi.Context, emu_api, oracle, _capi.LyraB200Error, pc.HostMem(), frames=2)
+
+
+def test_emu_device_entry_points(emu_api, oracle, sample1):
+    # every *_device call against its host-buffer twin and the oracle; 10 streams = one full tile and a partial one
+    pc.run_device_parity(_capi.Context, emu_api, oracle, pc.HostMem(), sample1, n=10, frames=10, check=[0, 4, 8, 9])
 
 
 def test_emu_full_duplex_threads(emu_api, oracle):

@@ -13,6 +13,34 @@ from lyra_b200 import _capi
 pytestmark = pytest.mark.gpu
 
 
+class TorchMem:
+    """Device buffers for the device-resident entry points: torch CUDA tensors, allocated, filled and read on one torch stream
+    of their own, which is also the stream the cases install in their contexts (lyra_b200_set_stream) - so every copy and every
+    library call is ordered on that stream and reading a result back needs no other synchronisation.  (Not the default stream:
+    its handle is 0, which lyra_b200_set_stream takes as "the context's own stream".)"""
+
+    def __init__(self):
+        import torch
+        self.torch = torch
+        self.s = torch.cuda.Stream()
+        self.stream = self.s.cuda_stream
+
+    def zeros(self, shape, dtype):
+        with self.torch.cuda.stream(self.s):
+            return self.torch.zeros(shape, dtype=getattr(self.torch, np.dtype(dtype).name), device="cuda")
+
+    def ptr(self, t):
+        return t.data_ptr()
+
+    def put(self, t, a):
+        with self.torch.cuda.stream(self.s):
+            t.copy_(self.torch.from_numpy(np.ascontiguousarray(a)))
+
+    def get(self, t):
+        with self.torch.cuda.stream(self.s):
+            return t.cpu().numpy()
+
+
 def test_codec_parity_speech_with_loss(gpu_api, oracle, sample1):
     pc.run_codec_parity(_capi.Context, gpu_api, oracle, max_streams=100, stream_ids=[0, 5, 17, 31, 32, 64, 99],
                         frames=60, bits=64, wav=sample1, loss_every=6)
@@ -121,7 +149,7 @@ def test_decode_track_noise_sparse_and_dense(gpu_api, oracle, sample1):
 
 
 def test_role_contexts(gpu_api, oracle):
-    pc.run_role_contexts(_capi.Context, gpu_api, oracle, _capi.LyraB200Error, frames=20)
+    pc.run_role_contexts(_capi.Context, gpu_api, oracle, _capi.LyraB200Error, TorchMem(), frames=20)
 
 
 @pytest.mark.parametrize("mode", ["exact", "tensor"])
@@ -429,3 +457,277 @@ def test_integration_criterion_other_sample_rates(gpu_api, oracle, rate):
     worst = pc.run_integration_other_rates(_capi.Context, gpu_api, oracle, rate=rate, wav=wav)
     print("integration LSD at %d Hz: worst hop %.3f" % (rate, worst))
     assert worst < 2.0
+
+
+# ---- the device-resident entry points: the path bench.py times ----
+
+@pytest.mark.parametrize("mode", ["exact", "tensor"])
+def test_device_entry_points(gpu_api, oracle, sample1, mode):
+    # every *_device call against its host-buffer twin (all 1100 streams) and the oracle; 1100 streams = 138 tiles, the last one
+    # partial, and split 2 engages (>= 128 tiles): the check streams sit at the edges of both sub-batches
+    pc.run_device_parity(_capi.Context, gpu_api, oracle, TorchMem(), sample1, n=1100, frames=12, check=[0, 551, 552, 1097, 1099],
+                         decoder_mode=mode, split=2)
+
+
+def _torch():
+    import torch
+    return torch
+
+
+@pytest.mark.parametrize("workload,mode,split", [("codec", "exact", 2), ("codec", "tensor", 3),
+                                                 ("decode_plc", "exact", 3), ("decode_plc", "tensor", 2)])
+def test_bench_device_schedule(gpu_api, oracle, workload, mode, split):
+    """bench.py's device-resident pass (measure -> run_device) at a size where its sub-batches engage: G = 2 context pairs over
+    slices of shared buffers, caller streams at priorities -1 / 0, encoder -> decoder events, 12 hops over 8 rotating slots queued
+    with no host synchronisation.  2 x 1540 streams: 193 tiles per context, the last one partial, so a slice's last tile ends in
+    the middle of the shared buffer.  Every hop's output goes to its own buffer; all streams are compared with host-buffer calls
+    on a reference context per group, the streams at the slice edges with the oracle."""
+    torch = _torch()
+    plc = workload == "decode_plc"
+    G, m, NBUF, hops, bits = 2, 1540, 8, 12, 64
+    n, P = G * m, _capi.packet_bytes(bits)
+    tol = pc.TENSOR_PCM_TOL_LSB if mode == "tensor" else 0
+    rng = np.random.default_rng(17)
+    host_pcm = [pc.synth_pcm(rng, n, "noise" if b % 4 else "loud") for b in range(NBUF)]
+    d_pcm = [torch.from_numpy(x).cuda() for x in host_pcm]
+    d_pks = [torch.zeros((n, P), dtype=torch.uint8, device="cuda") for _ in range(NBUF)]
+    d_out = [torch.full((n, 320), 0x5A5A, dtype=torch.int16, device="cuda") for _ in range(hops)]
+    d_flags = [torch.full((n,), 0xAA, dtype=torch.uint8, device="cuda") for _ in range(hops)]
+    pk_of_hop = [torch.zeros((n, P), dtype=torch.uint8, device="cuda") for _ in range(hops)]
+    edges = [0, m - 1, m, n - 1]
+    if plc:
+        # the workload's packets come from an encoder over the 8 input slots; bursts of 7 lost hops (slots 1..7) reach comfort
+        # noise on every 5th stream and on the edge streams, the others lose packets at random
+        tmp = _capi.Context(n, roles="encoder")
+        h_pks = [tmp.encode(x, bits) for x in host_pcm]
+        tmp.close()
+        for b in range(NBUF):
+            d_pks[b].copy_(torch.from_numpy(h_pks[b]))
+        burst = np.zeros(n, bool)
+        burst[::5] = True
+        burst[edges] = True
+        h_masks = [((rng.random(n) >= 0.15) & ~(burst & (b > 0))).astype(np.uint8) for b in range(NBUF)]
+        d_masks = [torch.from_numpy(x).cuda() for x in h_masks]
+    groups = []
+    for g in range(G):
+        e_ = None if plc else _capi.Context(m, roles="encoder")
+        d_ = _capi.Context(m, roles="decoder")
+        d_.set_decoder_mode(mode)
+        gx, gy = torch.cuda.Stream(priority=-1), torch.cuda.Stream(priority=0)
+        d_.set_priority(0)
+        d_.set_stream(gy.cuda_stream)
+        d_.set_split(split)
+        if e_:
+            e_.set_priority(-1)
+            e_.set_stream(gx.cuda_stream)
+            e_.set_split(split)
+        groups.append((e_, d_, gx, gy))
+    ev_pk = [[torch.cuda.Event() for _ in range(NBUF)] for _ in range(G)]
+    ev_free = [[torch.cuda.Event() for _ in range(NBUF)] for _ in range(G)]
+    torch.cuda.synchronize()
+    for i in range(hops):
+        b = i % NBUF
+        for g, (e_, d_, gx, gy) in enumerate(groups):
+            off = g * m
+            if plc:
+                d_.decode_plc_device(m, d_pks[b].data_ptr() + off * P, d_masks[b].data_ptr() + off, bits,
+                                     d_out[i].data_ptr() + off * 640, d_flags[i].data_ptr() + off)
+                continue
+            if i >= NBUF:
+                gx.wait_event(ev_free[g][b])                   # the ring slot's previous packets have been decoded
+            e_.encode_device(m, d_pcm[b].data_ptr() + off * 640, bits, d_pks[b].data_ptr() + off * P)
+            ev_pk[g][b].record(gx)
+            gy.wait_event(ev_pk[g][b])
+            d_.decode_device(m, d_pks[b].data_ptr() + off * P, 0, bits, d_out[i].data_ptr() + off * 640)
+            with torch.cuda.stream(gy):                        # keep this hop's packets before the slot is reused
+                pk_of_hop[i][off:off + m].copy_(d_pks[b][off:off + m])
+            ev_free[g][b].record(gy)
+    torch.cuda.synchronize()
+    outs = [x.cpu().numpy() for x in d_out]
+    flags = [x.cpu().numpy() for x in d_flags]
+    pks = [x.cpu().numpy() for x in pk_of_hop]
+    # reference: one context per group (the comfort-noise seed of a stream is the context's seed plus its id in that context)
+    refs = [(None if plc else _capi.Context(m, roles="encoder"), _capi.Context(m, roles="decoder")) for _ in range(G)]
+    for _, rd in refs:
+        rd.set_decoder_mode(mode)
+    oracles = {s: (oracle.Decoder(_capi.MODEL_DIR, cng_seed=s % m) if plc else oracle.Codec(_capi.MODEL_DIR)) for s in edges}
+    seen_cn = False
+    for i in range(hops):
+        b = i % NBUF
+        for g, (re, rd) in enumerate(refs):
+            sl = slice(g * m, (g + 1) * m)
+            if plc:
+                want, cn = rd.decode_plc(h_pks[b][sl], bits, received=h_masks[b][sl])
+                assert np.array_equal(flags[i][sl], cn.astype(np.uint8)), (i, g)
+                seen_cn |= bool(cn.any())
+            else:
+                pk = re.encode(host_pcm[b][sl], bits)
+                assert np.array_equal(pks[i][sl], pk), "packets of hop %d group %d" % (i, g)
+                want = rd.decode(pk, bits)
+            bad = np.nonzero((outs[i][sl] != want).any(axis=1))[0]
+            assert bad.size == 0, "PCM of hop %d group %d differs from host-buffer calls at streams %s" % (i, g, (bad + g * m)[:8])
+        for s in edges:
+            if plc:
+                if h_masks[b][s]:
+                    assert oracles[s].set_encoded_packet(bytes(h_pks[b][s]))
+                opcm = oracles[s].decode_samples(320)
+                assert bool(flags[i][s]) == oracles[s].is_comfort_noise(), (i, s)
+            else:
+                opkt, _, _ = oracles[s].encode(host_pcm[b][s], bits)
+                assert bytes(pks[i][s]) == opkt, (i, s)
+                opcm, _, _ = oracles[s].decode(opkt, bits)
+            d = int(np.abs(outs[i][s].astype(int) - opcm.astype(int)).max())
+            assert d <= tol, "hop %d stream %d: max |PCM - oracle| %d" % (i, s, d)
+    assert not plc or seen_cn
+    for c in [c for grp in groups for c in grp[:2]] + [c for r in refs for c in r]:
+        if c is not None:
+            c.close()
+
+
+def _device_pairs(n, split):
+    """One context per *_device entry point and its host-buffer twin, dense calls over n streams."""
+    roles = dict(enc="encoder", dec="decoder", trk="decoder", nz="encoder", plc="decoder", dtx="encoder")
+    dev = {k: _capi.Context(n, roles=r) for k, r in roles.items()}
+    host = {k: _capi.Context(n, roles=r) for k, r in roles.items()}
+    for c in dev.values():
+        c.set_split(split)
+    return dev, host
+
+
+def test_device_calls_follow_the_caller_stream(gpu_api):
+    """lyra_b200_set_stream: the calls read their inputs in stream order on the installed stream.  The caller stream fills the
+    input buffer, makes the call, then at once overwrites the buffer with the next hop's input - no host synchronisation
+    anywhere; a spin queued first keeps the caller stream far behind the host, so a call that read its input on any other stream
+    would read it before it was written.  Results must be those of the un-overwritten inputs."""
+    torch = _torch()
+    n, bits, hops = 1024, 120, 4
+    P = _capi.packet_bytes(bits)
+    rng = np.random.default_rng(8)
+    pcm = [pc.synth_pcm(rng, n) for _ in range(hops)]
+    d_src = [torch.from_numpy(x).cuda() for x in pcm]
+    trash = torch.from_numpy(pc.synth_pcm(rng, n, "loud")).cuda()
+    enc = _capi.Context(n, roles="encoder")
+    dec = _capi.Context(n, roles="decoder")
+    ref = _capi.Context(n)
+    s = torch.cuda.Stream()
+    for c in (enc, dec):
+        c.set_split(2)
+        c.set_stream(s.cuda_stream)
+    buf = torch.zeros((n, 320), dtype=torch.int16, device="cuda")
+    pk_buf = torch.zeros((n, P), dtype=torch.uint8, device="cuda")
+    pks = [torch.zeros((n, P), dtype=torch.uint8, device="cuda") for _ in range(hops)]
+    outs = [torch.zeros((n, 320), dtype=torch.int16, device="cuda") for _ in range(hops)]
+    torch.cuda.synchronize()
+    with torch.cuda.stream(s):
+        torch.cuda._sleep(50_000_000)
+        for f in range(hops):
+            buf.copy_(d_src[f])
+            enc.encode_device(n, buf.data_ptr(), bits, pks[f].data_ptr())
+            buf.copy_(d_src[f + 1] if f + 1 < hops else trash)
+            pk_buf.copy_(pks[f])
+            dec.decode_device(n, pk_buf.data_ptr(), 0, bits, outs[f].data_ptr())
+            pk_buf.zero_()
+    s.synchronize()
+    for f in range(hops):
+        want_pk = ref.encode(pcm[f], bits)
+        assert np.array_equal(pks[f].cpu().numpy(), want_pk), "encode_device read an overwritten input (hop %d)" % f
+        assert np.array_equal(outs[f].cpu().numpy(), ref.decode(want_pk, bits)), "decode_device read overwritten packets (hop %d)" % f
+    for c in (enc, dec, ref):
+        c.close()
+
+
+def test_device_calls_do_not_wait_for_the_gpu(gpu_api, sample1):
+    """The *_device calls are asynchronous on the installed stream (include/lyra_b200.h, DESIGN.md section 4): with a spin of a
+    few tens of ms queued ahead on the caller stream, every dense call returns while the stream is still busy.  Ordering only:
+    the results, read after synchronising, equal the host-buffer twins'."""
+    torch = _torch()
+    n, bits = 1024, 64
+    P = _capi.packet_bytes(bits)
+    dev, host = _device_pairs(n, 2)
+    s = torch.cuda.Stream()
+    for c in dev.values():
+        c.set_stream(s.cuda_stream)
+    pcm = np.stack([sample1[(320 * (7 * k)) % (len(sample1) - 320):][:320] for k in range(n)]).copy()
+    pcm[::3] = 0
+    rec = (np.arange(n) % 5 != 0).astype(np.uint8)
+    d_pcm, d_rec = torch.from_numpy(pcm).cuda(), torch.from_numpy(rec).cuda()
+    d_pk = torch.zeros((n, P), dtype=torch.uint8, device="cuda")
+    d_out = torch.zeros((n, 320), dtype=torch.int16, device="cuda")
+    d_flags = torch.zeros(n, dtype=torch.uint8, device="cuda")
+    d_est = torch.zeros((n, 160), dtype=torch.float32, device="cuda")
+    calls = [("encode_device", lambda: dev["enc"].encode_device(n, d_pcm.data_ptr(), bits, d_pk.data_ptr()),
+              lambda: host["enc"].encode(pcm, bits), lambda: d_pk),
+             ("decode_device", lambda: dev["dec"].decode_device(n, d_pk.data_ptr(), d_rec.data_ptr(), bits, d_out.data_ptr()),
+              lambda: host["dec"].decode(want["encode_device"], bits, received=rec), lambda: d_out),
+             ("decode_track_noise_device", lambda: dev["trk"].decode_track_noise_device(n, d_pk.data_ptr(), d_rec.data_ptr(), bits,
+                                                                                          d_out.data_ptr(), d_flags.data_ptr()),
+              lambda: host["trk"].decode_track_noise(want["encode_device"], bits, received=rec)[0], lambda: d_out),
+             ("noise_update_device", lambda: dev["nz"].noise_update_device(n, d_pcm.data_ptr(), d_rec.data_ptr(), d_flags.data_ptr(),
+                                                                           d_est.data_ptr()),
+              lambda: host["nz"].noise_update(pcm, update_mask=rec)[1], lambda: d_est),
+             ("decode_plc_device", lambda: dev["plc"].decode_plc_device(n, d_pk.data_ptr(), d_rec.data_ptr(), bits, d_out.data_ptr(),
+                                                                        d_flags.data_ptr()),
+              lambda: host["plc"].decode_plc(want["encode_device"], bits, received=rec)[0], lambda: d_out),
+             ("encode_dtx_device", lambda: dev["dtx"].encode_dtx_device(n, d_pcm.data_ptr(), bits, d_pk.data_ptr(), d_flags.data_ptr()),
+              lambda: host["dtx"].encode_dtx(pcm, bits)[0], lambda: d_pk)]
+    torch.cuda.synchronize()
+    want = {}
+    for hop in range(2):                   # hop 0 warms every call up (first launches, stream maps); hop 1 is checked
+        for name, call, twin, result in calls:
+            with torch.cuda.stream(s):
+                if hop:
+                    torch.cuda._sleep(50_000_000)
+                call()
+            if hop:
+                assert not s.query(), "%s waited for the GPU" % name
+            s.synchronize()
+            want[name] = twin()
+            assert np.array_equal(result().cpu().numpy(), want[name]), "%s (hop %d) != its host-buffer twin" % (name, hop)
+    for c in list(dev.values()) + list(host.values()):
+        c.close()
+
+
+@pytest.mark.parametrize("workload,mode", [("codec", "exact"), ("codec", "tensor"), ("decode_plc", "exact"), ("decode_plc", "tensor")])
+def test_bench_dumps_match_the_oracle(gpu_api, oracle, tmp_path, workload, mode):
+    """bench.py --dump-outputs at a small size against the oracle replaying the same seeded schedule: the warm-up hops, then the
+    timed hops restarting at hop 0, hop i feeding input slot i % 8 (bench.synth_pcm_np); decode_plc: packets of a fresh encoder
+    over slots 0..7, the received mask of slot b = the b-th Bernoulli(1 - loss) draw of default_rng(1234 + rank) (bench.py, measure),
+    comfort-noise seed = the context's (0) + the stream's id in its group."""
+    import subprocess
+    import sys
+    import bench
+    from conftest import ROOT
+    n, groups, steps, hps, warmup, bits, loss = 64, 2, 2, 2, 3, 64, 0.1
+    out = tmp_path / "dump"
+    cmd = [sys.executable] + (["-s"] if sys.flags.no_user_site else []) + [
+        os.path.join(ROOT, "bench.py"), "--gpus", "1", "--streams", str(n), "--groups", str(groups), "--split", "2",
+        "--steps", str(steps), "--hops-per-step", str(hps), "--warmup", str(warmup), "--no-cpu-baseline", "--no-other-configs",
+        "--workload", workload, "--loss", str(loss), "--decoder-mode", mode, "--dump-outputs", str(out)]
+    r = subprocess.run(cmd, capture_output=True, text=True, timeout=600, cwd=str(tmp_path))
+    assert r.returncode == 0, r.stdout[-2000:] + r.stderr[-4000:]
+    json.loads(r.stdout.strip().splitlines()[-1])
+    dump = {name: np.load(str(out / (name + ".npy"))) for name in (("pcm", "flags") if workload == "decode_plc" else ("pcm", "packets"))}
+    hop_order = list(range(max(3, max(3, warmup) * hps))) + list(range(steps * hps))
+    host = bench.synth_pcm_np(n, 8, bench.SEED, "noise")
+    m = n // groups
+    tol = pc.TENSOR_PCM_TOL_LSB if mode == "tensor" else 0
+    mrng = np.random.default_rng(1234 + 0)                # rank 0
+    masks = [(mrng.random(n) >= loss).astype(np.uint8) for _ in range(8)]
+    for s in (0, m - 1, m, n - 1):
+        if workload == "decode_plc":
+            enc = oracle.Encoder(_capi.MODEL_DIR)
+            pks = [enc.encode(host[b][s], bits) for b in range(8)]
+            dec = oracle.Decoder(_capi.MODEL_DIR, cng_seed=s % m)
+            for i in hop_order:
+                if masks[i % 8][s]:
+                    assert dec.set_encoded_packet(pks[i % 8])
+                pcm = dec.decode_samples(320)
+            assert dump["flags"][s] == float(dec.is_comfort_noise()), s
+        else:
+            codec = oracle.Codec(_capi.MODEL_DIR)
+            for i in hop_order:
+                pkt, _, _ = codec.encode(host[i % 8][s], bits)
+                pcm, _, _ = codec.decode(pkt, bits)
+            assert bytes(dump["packets"][s].astype(np.uint8)) == pkt, s
+        d = int(np.abs(dump["pcm"][s].astype(int) - pcm.astype(int)).max())
+        assert d <= tol, "stream %d: max |dumped PCM - oracle| %d" % (s, d)
