@@ -113,7 +113,9 @@ RvqDecodeKernel(const uint8_t* __restrict__ blob, RvqParams P, const uint8_t* __
 
 // ------------------------------------------------------------------------------------------------
 // Reset the streaming state of selected streams to the reference's CALL_ONCE initial values
-// (all-zero resource variables; int8 rings hold the zero point of their tensor).
+// (all-zero resource variables; int8 rings hold the zero point of their tensor).  state[tile][unit][S] with
+// tile = stream / S, lane = stream % S; S = 1 is a row-major [stream][units] buffer.  init == nullptr: all zero;
+// n18 == nullptr: the state has no hop counter.
 __global__ void __launch_bounds__(256)
 ResetStateKernel(uint32_t* __restrict__ state, const uint32_t* __restrict__ init, int units, int S,
                  const int* __restrict__ streams, int nstreams, int* __restrict__ n18) {
@@ -122,8 +124,8 @@ ResetStateKernel(uint32_t* __restrict__ state, const uint32_t* __restrict__ init
   const int stream = streams ? streams[k] : k;
   const int tile = stream / S, lane = stream % S;
   uint32_t* st = state + (size_t)tile * units * S + lane;
-  for (int u = (int)threadIdx.x; u < units; u += (int)blockDim.x) st[(size_t)u * S] = init[u];
-  if (threadIdx.x == 0) n18[stream] = 0;
+  for (int u = (int)threadIdx.x; u < units; u += (int)blockDim.x) st[(size_t)u * S] = init ? init[u] : 0u;
+  if (n18 && threadIdx.x == 0) n18[stream] = 0;
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -147,7 +147,97 @@ def run_error_paths(Context, api, LyraB200Error):
     assert fails(lambda: ctx.encode(pcm, 64, stream_ids=np.array([1, 8], dtype=np.int32)))   # id out of range
     assert fails(lambda: ctx.encode(np.zeros((9, 320), np.int16), 64))              # more rows than streams
     assert fails(lambda: ctx.logmel(pcm, num_mel_bins=80))
+    # every call that takes stream ids refuses ids out of range and, except reset and the control-state calls, repeated ids
+    pk = np.zeros((2, 8), dtype=np.uint8)
+    takes_ids = {
+        "encode": lambda ids: ctx.encode(pcm, 64, stream_ids=ids),
+        "decode": lambda ids: ctx.decode(pk, 64, stream_ids=ids),
+        "extract_features": lambda ids: ctx.extract_features(pcm, stream_ids=ids),
+        "generate": lambda ids: ctx.generate(np.zeros((2, 64), np.float32), stream_ids=ids),
+        "logmel": lambda ids: ctx.logmel(pcm, stream_ids=ids),
+        "noise_update": lambda ids: ctx.noise_update(pcm, stream_ids=ids),
+        "noise_estimate": lambda ids: ctx.noise_estimate(stream_ids=ids),
+        "decode_track_noise": lambda ids: ctx.decode_track_noise(pk, 64, stream_ids=ids),
+        "decode_plc": lambda ids: ctx.decode_plc(pk, 64, stream_ids=ids),
+        "cng_generate": lambda ids: ctx.cng_generate(np.zeros((2, 160), np.float32), stream_ids=ids),
+        "encode_dtx": lambda ids: ctx.encode_dtx(pcm, 64, stream_ids=ids),
+        "resample": lambda ids: ctx.resample(np.zeros((2, 160), np.int16), 8000, True, stream_ids=ids),
+    }
+    repeats_ok = {
+        "reset": lambda ids: ctx.reset(stream_ids=ids),
+        "plc_state": lambda ids: ctx.plc_state(stream_ids=ids),
+        "set_plc_state": lambda ids: ctx.set_plc_state([(0, 0, -1)] * len(ids), stream_ids=ids),
+    }
+    for name, call in list(takes_ids.items()) + list(repeats_ok.items()):
+        for bad in ([1, 8], [-1, 2]):
+            assert fails(lambda: call(np.array(bad, dtype=np.int32))), "%s accepted stream ids %s" % (name, bad)
+        if name in takes_ids:
+            assert fails(lambda: call(np.array([3, 3], dtype=np.int32))), "%s accepted a repeated stream id" % name
+        else:
+            call(np.array([3, 3], dtype=np.int32))
     ctx.close()
+
+
+def _every_stateful_call(ctx, f, ids, wav, bits):
+    """Hop f of every call that advances per-stream state, on streams `ids`; the inputs depend on f only.  Decode_plc receives hop 0,
+    loses hops 1..7 (long enough to reach comfort noise) and then every other stream's packets.  Returns {name: per-stream rows}."""
+    n = len(ids)
+    rng = np.random.default_rng(100 + f)
+    pcm = np.stack([wav[(320 * (f + 9 * k + 30)) % (len(wav) - 320):][:320] for k in range(n)]).copy()
+    quiet = pcm.copy()
+    quiet[::2] = 0                                       # DTX and the estimators' noise branch on every other stream
+    out = {}
+    pk = ctx.encode(pcm, bits, stream_ids=ids)
+    out["packets"] = pk
+    out["pcm"] = ctx.decode(pk, bits, stream_ids=ids, received=(np.arange(n) + f) % 4 != 0)
+    plc_rec = np.ones(n, np.uint8) if f == 0 else (np.arange(n) % 2).astype(np.uint8) if f >= 8 else np.zeros(n, np.uint8)
+    out["plc_pcm"], out["comfort_noise"] = ctx.decode_plc(pk, bits, stream_ids=ids, received=plc_rec)
+    out["plc_state"] = ctx.plc_state(stream_ids=ids)
+    out["dtx_packets"], out["dtx_bytes"] = ctx.encode_dtx(quiet, bits, stream_ids=ids)
+    out["logmel_bank0"] = ctx.logmel(pcm, 160, bank=0, stream_ids=ids)
+    out["logmel_bank1"] = ctx.logmel(quiet, 64, bank=1, stream_ids=ids)
+    out["is_noise"], out["noise_estimate"] = ctx.noise_update(quiet, stream_ids=ids)
+    out["cng"] = ctx.cng_generate(rng.uniform(0.62, 1.2, size=(n, 160)).astype(np.float32), stream_ids=ids)
+    chunk = (960, 7, 955, 480, 13, 960)[f % 6]           # ragged chunks leave the resamplers mid-phase
+    out["resample_in"] = ctx.resample(rng.integers(-20000, 20000, size=(n, chunk)).astype(np.int16), 48000, True, stream_ids=ids)
+    out["resample_out"] = ctx.resample(pcm[:, :320 - 17 * (f % 5)], 8000, False, stream_ids=ids)
+    return out
+
+
+def run_reset_restores_every_stream_state(Context, api, wav, *, max_streams=16, ids=(1, 6, 9, 14), reset_ids=(9, 1, 9), dense_n=8,
+                                          hops=9, bits=64, cng_seed=3):
+    """lyra_b200_reset restores all per-stream state: three contexts run the same history through every stateful call, then one
+    resets `reset_ids` (an id listed twice) and one resets streams 0..dense_n-1.  On the next hop a reset stream must equal a fresh
+    context's first hop and every other stream the twin that was not reset, in every output and in the control state, bit for bit."""
+    ids = np.asarray(ids, dtype=np.int32)
+
+    def make():
+        c = Context(max_streams, capi=api)
+        c.set_cng_seed(cng_seed)
+        return c
+    sparse, dense, twin = make(), make(), make()
+    seen_cn = seen_dtx = False
+    for f in range(hops):
+        for c in (sparse, dense, twin):
+            o = _every_stateful_call(c, f, ids, wav, bits)
+        seen_cn |= bool(o["comfort_noise"].any())
+        seen_dtx |= bool((o["dtx_bytes"] == 0).any())
+    assert seen_cn and seen_dtx, "the history must reach comfort noise and DTX"
+    sparse.reset(np.asarray(reset_ids, dtype=np.int32))
+    dense.reset(n=dense_n)
+    fresh = make()
+    twin_state = twin.plc_state(stream_ids=ids)
+    want = {True: _every_stateful_call(fresh, hops, ids, wav, bits), False: _every_stateful_call(twin, hops, ids, wav, bits)}
+    for c, was_reset, how in ((sparse, np.isin(ids, reset_ids), "reset(%s)" % list(reset_ids)), (dense, ids < dense_n, "reset(n=%d)" % dense_n)):
+        assert was_reset.any() and not was_reset.all()
+        st = c.plc_state(stream_ids=ids)
+        got = _every_stateful_call(c, hops, ids, wav, bits)
+        for k, s in enumerate(ids):
+            assert tuple(st[k]) == ((0, 0, -1) if was_reset[k] else tuple(twin_state[k])), "control state of stream %d after %s" % (s, how)
+            for name, rows in got.items():
+                assert np.array_equal(rows[k], want[bool(was_reset[k])][name][k]), "%s of stream %d after %s" % (name, s, how)
+    for c in (sparse, dense, twin, fresh):
+        c.close()
 
 
 def run_logmel_parity(Context, api, O, wav, *, n=4, frames=4, tol=0.0):

@@ -40,6 +40,11 @@ def test_emu_reset_and_isolation(emu_api, oracle):
     pc.run_reset_and_isolation(_capi.Context, emu_api, oracle)
 
 
+def test_emu_reset_restores_every_stream_state(emu_api, sample1):
+    # ids 1 / 6 in tile 0 and 9 / 14 in tile 1: every tile holds a reset stream and one that is not reset
+    pc.run_reset_restores_every_stream_state(_capi.Context, emu_api, sample1)
+
+
 def test_emu_error_paths(emu_api):
     pc.run_error_paths(_capi.Context, emu_api, _capi.LyraB200Error)
 

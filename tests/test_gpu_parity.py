@@ -130,6 +130,11 @@ def test_reset_and_isolation(gpu_api, oracle):
     pc.run_reset_and_isolation(_capi.Context, gpu_api, oracle)
 
 
+def test_reset_restores_every_stream_state(gpu_api, sample1):
+    pc.run_reset_restores_every_stream_state(_capi.Context, gpu_api, sample1, max_streams=64, ids=(1, 6, 9, 14, 33, 40, 63),
+                                             reset_ids=(40, 9, 1, 9), dense_n=16)
+
+
 def test_error_paths(gpu_api):
     pc.run_error_paths(_capi.Context, gpu_api, _capi.LyraB200Error)
 
@@ -685,6 +690,43 @@ def test_device_calls_do_not_wait_for_the_gpu(gpu_api, sample1):
             assert np.array_equal(result().cpu().numpy(), want[name]), "%s (hop %d) != its host-buffer twin" % (name, hop)
     for c in list(dev.values()) + list(host.values()):
         c.close()
+
+
+def test_reset_follows_the_caller_stream(gpu_api):
+    """lyra_b200_reset on an installed caller stream runs behind the work already queued there: decode_plc_device hops with every
+    packet lost wait behind a spin on the caller stream, then a dense reset() is called.  Afterwards every stream's control state
+    is the initial (0, 0, -1), and the next hop equals a fresh context's first hop."""
+    torch = _torch()
+    n, bits, hops = 1024, 64, 6
+    P = _capi.packet_bytes(bits)
+    rng = np.random.default_rng(31)
+    pk = rng.integers(0, 256, size=(n, P), dtype=np.uint8)
+    rec = (np.arange(n) % 3 != 0).astype(np.uint8)
+    ctx = _capi.Context(n, roles="decoder")
+    fresh = _capi.Context(n, roles="decoder")
+    s = torch.cuda.Stream()
+    ctx.set_stream(s.cuda_stream)
+    d_pk, d_rec = torch.from_numpy(pk).cuda(), torch.from_numpy(rec).cuda()
+    d_lost = torch.zeros(n, dtype=torch.uint8, device="cuda")
+    d_out = torch.zeros((n, 320), dtype=torch.int16, device="cuda")
+    d_cn = torch.zeros(n, dtype=torch.uint8, device="cuda")
+    torch.cuda.synchronize()
+    with torch.cuda.stream(s):
+        torch.cuda._sleep(50_000_000)
+        for _ in range(hops):
+            ctx.decode_plc_device(n, d_pk.data_ptr(), d_lost.data_ptr(), bits, d_out.data_ptr(), d_cn.data_ptr())
+        ctx.reset()
+    st = ctx.plc_state(n)
+    bad = np.nonzero((st != np.array([0, 0, -1])).any(axis=1))[0]
+    assert bad.size == 0, "control state after reset: %s at streams %s" % (st[bad[0]], bad[:8])
+    with torch.cuda.stream(s):
+        ctx.decode_plc_device(n, d_pk.data_ptr(), d_rec.data_ptr(), bits, d_out.data_ptr(), d_cn.data_ptr())
+    s.synchronize()
+    want, want_cn = fresh.decode_plc(pk, bits, received=rec)
+    assert np.array_equal(d_out.cpu().numpy(), want) and np.array_equal(d_cn.cpu().numpy(), want_cn.astype(np.uint8))
+    assert np.array_equal(ctx.plc_state(n), fresh.plc_state(n))
+    ctx.close()
+    fresh.close()
 
 
 @pytest.mark.parametrize("workload,mode", [("codec", "exact"), ("codec", "tensor"), ("decode_plc", "exact"), ("decode_plc", "tensor")])
