@@ -76,6 +76,8 @@ class CApi:
             "lyra_b200_encode_dtx": (ci, [vp, vp, ci, vp, ci, vp, vp]),
             "lyra_b200_encode_dtx_device": (ci, [vp, ci, vp, ci, vp, vp]),
             "lyra_b200_resample": (ci, [vp, ci, vp, ci, ci, vp, ci, vp, ci, vp]),
+            "lyra_b200_set_sample_rate": (ci, [vp, ci]),
+            "lyra_b200_sample_rate": (ci, [vp]),
         }
         for name, (res, args) in sig.items():
             fn = getattr(L, name)   # AttributeError here = the library does not export the declared ABI
@@ -92,7 +94,8 @@ class CApi:
                "lyra_b200_decode_track_noise_device", "lyra_b200_set_split", "lyra_b200_set_blocking_sync", "lyra_b200_set_graphs", "lyra_b200_set_priority", "lyra_b200_graph_replays", "lyra_b200_set_decoder_mode", "lyra_b200_decoder_mode", "lyra_b200_launch_count", "lyra_b200_profile_enable",
                "lyra_b200_profile_read", "lyra_b200_noise_estimate", "lyra_b200_decode_plc", "lyra_b200_decode_plc_device",
                "lyra_b200_plc_get_state", "lyra_b200_plc_set_state", "lyra_b200_cng_generate", "lyra_b200_set_cng_seed",
-               "lyra_b200_encode_dtx", "lyra_b200_encode_dtx_device", "lyra_b200_resample"]
+               "lyra_b200_encode_dtx", "lyra_b200_encode_dtx_device", "lyra_b200_resample", "lyra_b200_set_sample_rate",
+               "lyra_b200_sample_rate"]
 
 
 _product = None
@@ -133,7 +136,7 @@ def packet_bytes(num_bits):
 
 
 class Context:
-    """One GPU context: weights + the streaming state of ``max_streams`` independent 16 kHz streams."""
+    """One GPU context: weights + the streaming state of ``max_streams`` independent streams (16 kHz unless set_sample_rate)."""
 
     ROLES = {"both": 3, "encoder": 1, "decoder": 2}
 
@@ -174,8 +177,22 @@ class Context:
             a = np.ascontiguousarray(stream_ids, dtype=np.int32)
             self._check(self.api.lib.lyra_b200_reset(self.h, _ptr(a), a.size))
 
+    def set_sample_rate(self, sample_rate_hz):
+        """External rate of encode / decode / decode_plc / encode_dtx / decode_track_noise and their *_device twins: 8000, 16000
+        (default), 32000 or 48000.  Their PCM rows then hold sample_rate_hz // 50 samples."""
+        self._check(self.api.lib.lyra_b200_set_sample_rate(self.h, int(sample_rate_hz)))
+
+    @property
+    def sample_rate(self):
+        return int(self.api.lib.lyra_b200_sample_rate(self.h))
+
+    @property
+    def hop(self):
+        """Samples per PCM row of the codec calls at the context's sample rate."""
+        return self.sample_rate // 50
+
     def encode(self, pcm, num_bits, stream_ids=None):
-        pcm = np.ascontiguousarray(pcm, dtype=np.int16).reshape(-1, HOP)
+        pcm = np.ascontiguousarray(pcm, dtype=np.int16).reshape(-1, self.hop)
         n = pcm.shape[0]
         ids = _ids(stream_ids, n)
         out = np.empty((n, packet_bytes(num_bits)), dtype=np.uint8)
@@ -187,7 +204,7 @@ class Context:
         n = packets.shape[0]
         ids = _ids(stream_ids, n)
         rec = _mask(received, n, "received")
-        out = np.empty((n, HOP), dtype=np.int16)
+        out = np.empty((n, self.hop), dtype=np.int16)
         self._check(self.api.lib.lyra_b200_decode(self.h, _ptr(ids), n, _ptr(packets), _ptr(rec), num_bits, _ptr(out)))
         return out
 
@@ -239,7 +256,7 @@ class Context:
         n = packets.shape[0]
         ids = _ids(stream_ids, n)
         rec = _mask(received, n, "received")
-        out = np.empty((n, HOP), dtype=np.int16)
+        out = np.empty((n, self.hop), dtype=np.int16)
         flags = np.empty(n, dtype=np.uint8)
         self._check(self.api.lib.lyra_b200_decode_track_noise(self.h, _ptr(ids), n, _ptr(packets), _ptr(rec), num_bits, _ptr(out), _ptr(flags)))
         return out, flags.astype(bool)
@@ -275,7 +292,7 @@ class Context:
         n = packets.shape[0]
         ids = _ids(stream_ids, n)
         rec = _mask(received, n, "received")
-        out = np.empty((n, HOP), dtype=np.int16)
+        out = np.empty((n, self.hop), dtype=np.int16)
         cn = np.empty(n, dtype=np.uint8)
         self._check(self.api.lib.lyra_b200_decode_plc(self.h, _ptr(ids), n, _ptr(packets), _ptr(rec), num_bits, _ptr(out), _ptr(cn)))
         return out, cn.astype(bool)
@@ -309,7 +326,7 @@ class Context:
 
     def encode_dtx(self, pcm, num_bits, stream_ids=None):
         """LyraEncoder::Encode with DTX -> (packets[n][P], packet_bytes[n]: P, or 0 for an empty (noise) packet)."""
-        pcm = np.ascontiguousarray(pcm, dtype=np.int16).reshape(-1, HOP)
+        pcm = np.ascontiguousarray(pcm, dtype=np.int16).reshape(-1, self.hop)
         n = pcm.shape[0]
         ids = _ids(stream_ids, n)
         out = np.empty((n, packet_bytes(num_bits)), dtype=np.uint8)

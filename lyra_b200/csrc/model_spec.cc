@@ -763,6 +763,8 @@ ModelSpec BuildModelSpec(const std::string& model_dir) {
   s.logmel64 = BuildLogMelParams(&s.blob, 16000, 320, 640, 64);
   s.cng = BuildCngParams(&s.blob, s.logmel160, 640);
   s.resampler = BuildResamplerParams(&s.blob);
+  const int ext_rates[3] = {8000, 32000, 48000};
+  for (int r = 0; r < 3; ++r) s.logmel160_ext[r] = BuildLogMelParams(&s.blob, ext_rates[r], 320, 640, 160);
   while (s.blob.size() % 256) s.blob.push_back(0);
   return s;
 }

@@ -19,6 +19,9 @@ struct ModelSpec {
   RvqParams rvq;
   LogMelParams logmel160;         // 16 kHz, hop 320, window 640, 160 mel bins (NoiseEstimator's extractor)
   LogMelParams logmel64;          // 64 mel bins (lyra_integration_test's extractor)
+  // the encoder-side (DTX) estimator's extractor at an external rate of 8 / 32 / 48 kHz: it is created for the external rate and
+  // fed the 16 kHz hop (lyra/lyra_encoder.cc:80-89), so only its mel bank differs from logmel160
+  LogMelParams logmel160_ext[3];
   ResamplerParams resampler;      // 8 / 32 / 48 kHz <-> 16 kHz filter banks
   CngParams cng;                  // comfort-noise generator + cross-fade tables (decoder PLC path)
   int num_features = 64;

@@ -209,23 +209,25 @@ NoiseReadKernel(const int* __restrict__ stream_ids, int n, const float* __restri
 // Resampler::Resample (lyra/resampler.cc:52-57) for n streams, `n_in` input samples each: int16 -> float, polyphase FIR over the
 // 35-tap delay line, ClipToInt16.  Arithmetic and tap order are oracle/resampler.c's (one separately rounded multiply and add per
 // tap, ascending input order).  Per-stream state: delay[34] (the last 34 input samples), pos = position of the next output relative
-// to the next input sample, in units of 1 / den input samples; rate = the external rate the state belongs to (a call at another
-// rate starts from the fully-primed state, like a fresh Resampler).  counts[slot] = outputs produced (they differ by at most one
-// between streams when down-sampling from different phases); out rows are `out_stride` samples apart.
+// to the next input sample, in units of 1 / den input samples; tag = the configuration the state belongs to (lyra_b200_resample:
+// the external rate; the codec path: the generation of the context's rate setting).  A call with another tag starts from the
+// fully-primed state, like a fresh Resampler; 0 (what lyra_b200_reset writes) never matches.  counts[slot] (may be nullptr) =
+// outputs produced (they differ by at most one between streams when down-sampling from different phases).  I/O arrays are indexed
+// by slot: block b handles slot slot_base + b of a call of n slots; in rows are n_in samples and out rows `out_stride` samples apart.
 __global__ void __launch_bounds__(128)
-ResampleKernel(const uint8_t* __restrict__ blob, ResamplerParams P, int pair, int rate, const int* __restrict__ stream_ids, int n,
+ResampleKernel(const uint8_t* __restrict__ blob, ResamplerParams P, int pair, int tag, const int* __restrict__ stream_ids, int n,
                const int16_t* __restrict__ in, int n_in, int16_t* __restrict__ out, int out_stride, int* __restrict__ counts,
-               int16_t* __restrict__ delay_state, int* __restrict__ pos_state) {
+               int16_t* __restrict__ delay_state, int* __restrict__ pos_state, int slot_base) {
   unsigned char* smem = LYRA_DYN_SMEM();
   float* x = reinterpret_cast<float*>(smem);              // [34 + n_in]: delay line followed by the new samples
-  const int slot = (int)blockIdx.x;
+  const int slot = slot_base + (int)blockIdx.x;
   if (slot >= n) return;
   const int stream = stream_ids ? stream_ids[slot] : slot;
   constexpr int T = kResamplerTaps;
   const int tid = (int)threadIdx.x, NT = (int)blockDim.x;
   int16_t* dl = delay_state + (size_t)stream * (T - 1);
-  int* ps = pos_state + (size_t)stream * 2;              // {pos, rate}
-  const bool fresh = ps[1] != rate;
+  int* ps = pos_state + (size_t)stream * 2;              // {pos, tag}
+  const bool fresh = ps[1] != tag;
   const int a0 = fresh ? 0 : ps[0];
   for (int i = tid; i < T - 1; i += NT) x[i] = fresh ? 0.0f : (float)dl[i];
   for (int i = tid; i < n_in; i += NT) x[T - 1 + i] = (float)in[(size_t)slot * n_in + i];
@@ -248,7 +250,11 @@ ResampleKernel(const uint8_t* __restrict__ blob, ResamplerParams P, int pair, in
   }
   __syncthreads();
   for (int i = tid; i < T - 1; i += NT) dl[i] = (int16_t)x[n_in + i];     // the last 34 samples of [delay | in]
-  if (tid == 0) { ps[0] = a0 + count * num - total; ps[1] = rate; counts[slot] = count; }
+  if (tid == 0) {
+    ps[0] = a0 + count * num - total;
+    ps[1] = tag;
+    if (counts) counts[slot] = count;
+  }
 }
 
 }  // namespace lyra_b200
