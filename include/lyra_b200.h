@@ -67,6 +67,31 @@ int lyra_b200_tile_streams(const lyra_b200_ctx* ctx);
  * lyra_b200_set_stream) behind the work already queued there; returns when the reset is done. */
 int lyra_b200_reset(lyra_b200_ctx* ctx, const int32_t* stream_ids, int n);
 
+/* ---- moving streams: between ids of one context, between contexts, between GPUs and processes ----------------------
+ * A stream's state is everything lyra_b200_reset restores plus lyra_b200_resample's delay lines (which reset keeps): the
+ * networks' state and hop counters, the log-mel banks, both noise estimators, the packet-loss control state, the comfort-noise
+ * generator (overlap-add buffer, hop counter and its phase key), both directions of lyra_b200_resample and the codec calls'
+ * converters.  A moved stream continues exactly as it would have at its old id - comfort noise included, when both contexts
+ * have the same lyra_b200_set_cng_seed.  Host-side state of the C++ adapters (include/lyra_b200/) is not part of it.
+ *
+ * Bytes of one stream's state record in this context (it depends on the context's roles); 0 when ctx is NULL. */
+int lyra_b200_stream_state_bytes(const lyra_b200_ctx* ctx);
+/* records[n][lyra_b200_stream_state_bytes]: the complete state of the listed streams (stream_ids == NULL: 0..n-1; an id may be
+ * listed more than once).  A record holds a header (format, roles, sample rate, a fingerprint of the loaded model) and the
+ * state.  Ordered on the installed stream behind the work queued there; returns when the records are in the caller's buffer. */
+int lyra_b200_export_streams(lyra_b200_ctx* ctx, const int32_t* stream_ids, int n, void* records);
+/* The inverse of export, into this context's streams stream_ids[k] (NULL: 0..n-1; distinct).  Every record is validated first:
+ * a record of another format, roles, sample rate or model, or a damaged one, fails the whole call with LYRA_B200_EINVAL and no
+ * stream changes.  Records may come from a context in the other decoder mode (the modes share their state); the stream then
+ * continues in this context's mode.  Ordered on the installed stream; returns when done. */
+int lyra_b200_import_streams(lyra_b200_ctx* ctx, const int32_t* stream_ids, int n, const void* records);
+/* Within one context: afterwards stream dst_ids[k] holds the state stream src_ids[k] had before the call; src_ids[k] == -1 is
+ * the state at creation (what lyra_b200_reset gives).  Sources keep their state.  Asynchronous like the *_device calls: queued
+ * on the installed stream, no host synchronisation.  LYRA_B200_EINVAL for ids out of range, a repeated id within src_ids (-1
+ * excepted) or within dst_ids, or an id that is both a source and a destination.  With it a server keeps its live calls on
+ * streams 0..n-1 of the *_device calls: when the call on stream h ends it copies stream n-1 into h and shrinks n. */
+int lyra_b200_copy_streams(lyra_b200_ctx* ctx, const int32_t* src_ids, const int32_t* dst_ids, int n);
+
 /* ---- fused codec calls: host buffers in, host buffers out ------------------------------------------ */
 
 /* The external sample rate of the fused codec calls (LyraEncoder::Create / LyraDecoder::Create's sample_rate_hz,
@@ -173,7 +198,8 @@ int lyra_b200_plc_set_state(lyra_b200_ctx* ctx, const int32_t* stream_ids, int n
 /* ComfortNoiseGenerator::RunConditioning + RunModel(320) (lyra/comfort_noise_generator.cc:74-119) for n streams:
  * features[n][160] (log-mel, e.g. a noise estimate) -> pcm[n][320].  Every stream owns an overlap-add buffer and a hop
  * counter (cleared by lyra_b200_reset).  The reference draws random phases from an unseeded generator (:103); here the phase
- * of bin i of hop h of stream s is a pure function of (seed + s, h, i) - reproducible, see oracle/comfort_noise.c. */
+ * of bin i of hop h of stream s is a pure function of (seed + s, h, i) - reproducible, see oracle/comfort_noise.c.  (A stream
+ * moved by lyra_b200_import_streams / lyra_b200_copy_streams keeps the key of its old id.) */
 int lyra_b200_cng_generate(lyra_b200_ctx* ctx, const int32_t* stream_ids, int n, const float* features, int16_t* pcm);
 int lyra_b200_set_cng_seed(lyra_b200_ctx* ctx, uint64_t seed);   /* default 0 */
 

@@ -78,6 +78,10 @@ class CApi:
             "lyra_b200_resample": (ci, [vp, ci, vp, ci, ci, vp, ci, vp, ci, vp]),
             "lyra_b200_set_sample_rate": (ci, [vp, ci]),
             "lyra_b200_sample_rate": (ci, [vp]),
+            "lyra_b200_stream_state_bytes": (ci, [vp]),
+            "lyra_b200_export_streams": (ci, [vp, vp, ci, vp]),
+            "lyra_b200_import_streams": (ci, [vp, vp, ci, vp]),
+            "lyra_b200_copy_streams": (ci, [vp, vp, vp, ci]),
         }
         for name, (res, args) in sig.items():
             fn = getattr(L, name)   # AttributeError here = the library does not export the declared ABI
@@ -95,7 +99,8 @@ class CApi:
                "lyra_b200_profile_read", "lyra_b200_noise_estimate", "lyra_b200_decode_plc", "lyra_b200_decode_plc_device",
                "lyra_b200_plc_get_state", "lyra_b200_plc_set_state", "lyra_b200_cng_generate", "lyra_b200_set_cng_seed",
                "lyra_b200_encode_dtx", "lyra_b200_encode_dtx_device", "lyra_b200_resample", "lyra_b200_set_sample_rate",
-               "lyra_b200_sample_rate"]
+               "lyra_b200_sample_rate", "lyra_b200_stream_state_bytes", "lyra_b200_export_streams", "lyra_b200_import_streams",
+               "lyra_b200_copy_streams"]
 
 
 _product = None
@@ -176,6 +181,33 @@ class Context:
         else:
             a = np.ascontiguousarray(stream_ids, dtype=np.int32)
             self._check(self.api.lib.lyra_b200_reset(self.h, _ptr(a), a.size))
+
+    # ---- moving streams (lyra_b200_export_streams / _import_streams / _copy_streams) ----
+    def stream_state_bytes(self):
+        return int(self.api.lib.lyra_b200_stream_state_bytes(self.h))
+
+    def export_streams(self, stream_ids=None, n=None):
+        """The complete state of the listed streams (default: 0..n-1, n = max_streams) -> uint8[n, stream_state_bytes()]."""
+        ids = None if stream_ids is None else np.ascontiguousarray(stream_ids, dtype=np.int32)
+        n = ids.size if ids is not None else (self.max_streams if n is None else n)
+        out = np.empty((n, self.stream_state_bytes()), dtype=np.uint8)
+        self._check(self.api.lib.lyra_b200_export_streams(self.h, _ptr(ids), n, _ptr(out)))
+        return out
+
+    def import_streams(self, records, stream_ids=None):
+        """Install exported records into streams `stream_ids` (default: 0..len(records)-1)."""
+        recs = np.ascontiguousarray(records, dtype=np.uint8).reshape(-1, self.stream_state_bytes())
+        n = recs.shape[0]
+        ids = _ids(stream_ids, n)
+        self._check(self.api.lib.lyra_b200_import_streams(self.h, _ptr(ids), n, _ptr(recs)))
+
+    def copy_streams(self, src_ids, dst_ids):
+        """Stream dst_ids[k] <- the state of stream src_ids[k] (-1: the state at creation); asynchronous on the installed stream."""
+        src = np.ascontiguousarray(src_ids, dtype=np.int32).reshape(-1)
+        dst = np.ascontiguousarray(dst_ids, dtype=np.int32).reshape(-1)
+        if src.size != dst.size:
+            raise ValueError("src_ids and dst_ids must have the same length")
+        self._check(self.api.lib.lyra_b200_copy_streams(self.h, _ptr(src), _ptr(dst), src.size))
 
     def set_sample_rate(self, sample_rate_hz):
         """External rate of encode / decode / decode_plc / encode_dtx / decode_track_noise and their *_device twins: 8000, 16000

@@ -129,6 +129,180 @@ ResetStateKernel(uint32_t* __restrict__ state, const uint32_t* __restrict__ init
 }
 
 // ------------------------------------------------------------------------------------------------
+// Per-stream state records: lyra_b200_export_streams (gather), _import_streams (scatter), _copy_streams (copy).  Every kernel is
+// one launch over all entries of the context's state list (blockIdx.y = entry) and 8 consecutive rows of the call per block
+// (blockIdx.x).  A tile-blocked entry (lanes = 8) is read / written with the 8 rows of a block on 8 consecutive threads, so rows
+// that are the 8 lanes of one tile move whole 32-byte tile rows; the records side goes through shared memory and moves whole
+// lines.  Row-major entries (lanes = 1) are contiguous per stream on both sides.
+//
+// Record = kStateHeaderWords header words, then the entries' words in list order (each entry: its `words` words, then its hop
+// counter if it has one).  Two kinds of words are not copied verbatim between contexts:
+//   kStateCodecRs{0,1}  {position, tag} of a codec converter: the tag is a per-context counter (ResampleKernel); the record
+//                       stores 0 in its place and "was live" (tag == the context's) in the header; import writes the
+//                       destination's tag for a live converter and 0 (restart primed) otherwise;
+//   kStateCng           {hop counter, key offset} (2 x u64) of a comfort-noise generator: the phases are drawn from
+//                       seed + stream + offset; the record stores 0 for the offset and the key stream + offset in the header,
+//                       import and copy set the offset so that the key travels with the stream.
+enum StreamStateKind { kStatePlain = 0, kStateCodecRs0 = 1, kStateCodecRs1 = 2, kStateCng = 3 };
+constexpr uint32_t kStateMagic = 0x5453594Cu;        // "LYST"
+constexpr uint32_t kStateVersion = 1;
+constexpr int kStateHeaderWords = 16;
+// header words: magic, version, record bytes, roles, sample rate, 0, model fingerprint (lo, hi), codec converter 0 / 1 live,
+// comfort-noise key (lo, hi), 0 x 4
+enum { kHdrMagic = 0, kHdrVersion, kHdrBytes, kHdrRoles, kHdrRate, kHdrZero5, kHdrModelLo, kHdrModelHi, kHdrLive0, kHdrLive1,
+       kHdrKeyLo, kHdrKeyHi };
+constexpr int kStateMaxEntries = 24;
+constexpr int kStateRows = 8;                        // rows of a call per block
+constexpr int kStateChunk = 1024;                    // rows per launch (the ids travel as kernel parameters)
+constexpr int kStateThreads = 256;
+constexpr int kStateSmemUnits = 256;                 // units per shared-memory pass of a tile-blocked entry
+constexpr int kStateSmemBytes = kStateRows * kStateSmemUnits * 4;
+
+struct StreamStateEntry {
+  uint32_t* state;
+  const uint32_t* init;          // one stream's initial words (nullptr: zero)
+  int* n18;                      // hop counter (nullptr: none)
+  int words, lanes, offset, kind;   // offset: first word of the entry in a record
+};
+struct StreamStateTable {
+  StreamStateEntry e[kStateMaxEntries];
+  int count, record_words;
+  uint32_t header[kStateHeaderWords];   // the context's constant header words (export)
+};
+// src: export / copy sources (-1 in a copy: the state at creation), dst: import / copy destinations
+struct StreamIdChunk { int n; int src[kStateChunk]; int dst[kStateChunk]; };
+
+__device__ __forceinline__ uint32_t* StateWord(const StreamStateEntry& e, int stream, int u) {
+  return e.lanes == 1 ? e.state + (size_t)stream * e.words + u
+                      : e.state + ((size_t)(stream / e.lanes) * e.words + u) * e.lanes + stream % e.lanes;
+}
+__device__ __forceinline__ unsigned long long StateU64(const StreamStateEntry& e, int stream, int u) {
+  return (unsigned long long)*StateWord(e, stream, u) | ((unsigned long long)*StateWord(e, stream, u + 1) << 32);
+}
+__device__ __forceinline__ uint32_t InitWord(const StreamStateEntry& e, int u) { return e.init ? e.init[u] : 0u; }
+
+// records[k] <- the state of stream ids.src[k]; tag = the context's codec converter tag
+__global__ void __launch_bounds__(kStateThreads)
+StreamStateGatherKernel(StreamStateTable T, StreamIdChunk ids, uint32_t* __restrict__ records, int tag) {
+  uint32_t* sm = reinterpret_cast<uint32_t*>(LYRA_DYN_SMEM());   // [kStateRows][kStateSmemUnits] (kStateSmemBytes)
+  const int r0 = (int)blockIdx.x * kStateRows, tid = (int)threadIdx.x;
+  const int rows = ids.n - r0 < kStateRows ? ids.n - r0 : kStateRows;
+  if (rows <= 0) return;
+  const int RW = T.record_words;
+  if ((int)blockIdx.y == T.count) {                  // the headers
+    if (tid >= rows) return;
+    const int s = ids.src[r0 + tid];
+    uint32_t* h = records + (size_t)(r0 + tid) * RW;
+    for (int i = 0; i < kStateHeaderWords; ++i) h[i] = T.header[i];
+    for (int i = 0; i < T.count; ++i) {
+      const StreamStateEntry& e = T.e[i];
+      if (e.kind == kStateCodecRs0 || e.kind == kStateCodecRs1)
+        h[kHdrLive0 + e.kind - kStateCodecRs0] = (int)*StateWord(e, s, 1) == tag ? 1u : 0u;
+      if (e.kind == kStateCng) {
+        const unsigned long long key = StateU64(e, s, 2) + (unsigned long long)s;
+        h[kHdrKeyLo] = (uint32_t)key;
+        h[kHdrKeyHi] = (uint32_t)(key >> 32);
+      }
+    }
+    return;
+  }
+  const StreamStateEntry e = T.e[blockIdx.y];
+  uint32_t* out = records + kStateHeaderWords + e.offset;
+  if (e.lanes == 1) {
+    for (int j = 0; j < rows; ++j) {
+      const uint32_t* st = e.state + (size_t)ids.src[r0 + j] * e.words;
+      uint32_t* o = out + (size_t)(r0 + j) * RW;
+      for (int u = tid; u < e.words; u += kStateThreads) {
+        const bool dropped = (e.kind == kStateCodecRs0 || e.kind == kStateCodecRs1) ? u == 1 : e.kind == kStateCng && u >= 2;
+        o[u] = dropped ? 0u : st[u];
+      }
+    }
+  } else {
+    const int j = tid % kStateRows, uu = tid / kStateRows;
+    const int s = j < rows ? ids.src[r0 + j] : 0;
+    for (int u0 = 0; u0 < e.words; u0 += kStateSmemUnits) {
+      const int cnt = e.words - u0 < kStateSmemUnits ? e.words - u0 : kStateSmemUnits;
+      if (j < rows)
+        for (int u = uu; u < cnt; u += kStateThreads / kStateRows) sm[j * kStateSmemUnits + u] = *StateWord(e, s, u0 + u);
+      __syncthreads();
+      for (int jj = 0; jj < rows; ++jj)
+        for (int u = tid; u < cnt; u += kStateThreads) out[(size_t)(r0 + jj) * RW + u0 + u] = sm[jj * kStateSmemUnits + u];
+      __syncthreads();
+    }
+  }
+  if (e.n18 && tid < rows) out[(size_t)(r0 + tid) * RW + e.words] = (uint32_t)e.n18[ids.src[r0 + tid]];
+}
+
+// stream ids.dst[k] <- records[k] (validated by the host); tag = the context's codec converter tag
+__global__ void __launch_bounds__(kStateThreads)
+StreamStateScatterKernel(StreamStateTable T, StreamIdChunk ids, const uint32_t* __restrict__ records, int tag) {
+  uint32_t* sm = reinterpret_cast<uint32_t*>(LYRA_DYN_SMEM());   // [kStateRows][kStateSmemUnits] (kStateSmemBytes)
+  const int r0 = (int)blockIdx.x * kStateRows, tid = (int)threadIdx.x;
+  const int rows = ids.n - r0 < kStateRows ? ids.n - r0 : kStateRows;
+  if (rows <= 0) return;
+  const int RW = T.record_words;
+  const StreamStateEntry e = T.e[blockIdx.y];
+  const uint32_t* in = records + kStateHeaderWords + e.offset;
+  if (e.lanes == 1) {
+    for (int j = 0; j < rows; ++j) {
+      const int d = ids.dst[r0 + j];
+      const uint32_t* h = records + (size_t)(r0 + j) * RW;
+      const uint32_t* x = in + (size_t)(r0 + j) * RW;
+      uint32_t* st = e.state + (size_t)d * e.words;
+      const unsigned long long off = (((unsigned long long)h[kHdrKeyHi] << 32) | h[kHdrKeyLo]) - (unsigned long long)d;
+      for (int u = tid; u < e.words; u += kStateThreads) {
+        uint32_t v = x[u];
+        if ((e.kind == kStateCodecRs0 || e.kind == kStateCodecRs1) && u == 1) v = h[kHdrLive0 + e.kind - kStateCodecRs0] ? (uint32_t)tag : 0u;
+        if (e.kind == kStateCng && u >= 2) v = u == 2 ? (uint32_t)off : (uint32_t)(off >> 32);
+        st[u] = v;
+      }
+    }
+  } else {
+    const int j = tid % kStateRows, uu = tid / kStateRows;
+    const int d = j < rows ? ids.dst[r0 + j] : 0;
+    for (int u0 = 0; u0 < e.words; u0 += kStateSmemUnits) {
+      const int cnt = e.words - u0 < kStateSmemUnits ? e.words - u0 : kStateSmemUnits;
+      for (int jj = 0; jj < rows; ++jj)
+        for (int u = tid; u < cnt; u += kStateThreads) sm[jj * kStateSmemUnits + u] = in[(size_t)(r0 + jj) * RW + u0 + u];
+      __syncthreads();
+      if (j < rows)
+        for (int u = uu; u < cnt; u += kStateThreads / kStateRows) *StateWord(e, d, u0 + u) = sm[j * kStateSmemUnits + u];
+      __syncthreads();
+    }
+  }
+  if (e.n18 && tid < rows) e.n18[ids.dst[r0 + tid]] = (int)in[(size_t)(r0 + tid) * RW + e.words];
+}
+
+// stream ids.dst[k] <- stream ids.src[k] within one context, lane to lane (sources and destinations are disjoint);
+// ids.src[k] = -1: the entry's initial image
+__global__ void __launch_bounds__(kStateThreads)
+StreamStateCopyKernel(StreamStateTable T, StreamIdChunk ids) {
+  const int r0 = (int)blockIdx.x * kStateRows, tid = (int)threadIdx.x;
+  const int rows = ids.n - r0 < kStateRows ? ids.n - r0 : kStateRows;
+  if (rows <= 0) return;
+  const StreamStateEntry e = T.e[blockIdx.y];
+  if (e.lanes == 1) {
+    for (int j = 0; j < rows; ++j) {
+      const int s = ids.src[r0 + j], d = ids.dst[r0 + j];
+      // the key offset moves with the stream: seed + s + off(s) == seed + d + off(d)
+      const unsigned long long off = e.kind == kStateCng && s >= 0 ? StateU64(e, s, 2) + (unsigned long long)s - (unsigned long long)d : 0ull;
+      for (int u = tid; u < e.words; u += kStateThreads) {
+        uint32_t v = s < 0 ? InitWord(e, u) : e.state[(size_t)s * e.words + u];
+        if (e.kind == kStateCng && u >= 2) v = u == 2 ? (uint32_t)off : (uint32_t)(off >> 32);
+        e.state[(size_t)d * e.words + u] = v;
+      }
+    }
+  } else {
+    const int j = tid % kStateRows, uu = tid / kStateRows;
+    if (j < rows) {
+      const int s = ids.src[r0 + j], d = ids.dst[r0 + j];
+      for (int u = uu; u < e.words; u += kStateThreads / kStateRows) *StateWord(e, d, u) = s < 0 ? InitWord(e, u) : *StateWord(e, s, u);
+    }
+  }
+  if (e.n18 && tid < rows) e.n18[ids.dst[r0 + tid]] = ids.src[r0 + tid] < 0 ? 0 : e.n18[ids.src[r0 + tid]];
+}
+
+// ------------------------------------------------------------------------------------------------
 // Log-mel spectrogram (LogMelSpectrogramExtractorImpl::Extract, lyra/log_mel_spectrogram_extractor_impl.cc:96-126).
 // One block of 128 threads per stream: periodic-Hann window over [previous hop, current hop], zero-padded 1024-point
 // radix-2 decimation-in-time FFT in double — the same butterflies, operand order and host-computed twiddles as the

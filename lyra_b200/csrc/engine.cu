@@ -53,15 +53,25 @@ struct lyra_b200_ctx {
   int device = 0, max_streams = 0, ntiles = 0, padded = 0;
   int roles = LYRA_B200_ROLE_ENCODER | LYRA_B200_ROLE_DECODER;   // which halves of the streaming state this context holds
   std::vector<void*> allocs;         // every device allocation of the context (lyra_b200_destroy frees them)
-  // the per-stream state lyra_b200_reset restores: `words` 4-byte words per stream at lane stride `lanes` (layout of
-  // ResetStateKernel), set to `init` (nullptr: zero); the hop counter `n18` (nullptr: none) goes back to 0
-  struct ResetEntry {
+  // Every piece of per-stream state, in one list that drives lyra_b200_reset, _export_streams, _import_streams and
+  // _copy_streams: `words` 4-byte words per stream at lane stride `lanes` (layout of ResetStateKernel), initial image `init`
+  // (nullptr: zero), hop counter `n18` (nullptr: none; initially 0).  `reset` = false: lyra_b200_reset leaves the entry alone
+  // (lyra_b200_resample's delay lines).  `kind` (StreamStateKind) marks the words a record does not carry verbatim; `check`
+  // is what import validates in a record's payload besides the hop counter.
+  enum Check { kCheckNone, kCheckPlc, kCheckResamplerPos };
+  struct StateEntry {
     uint32_t* state;
     int words, lanes;
     const uint32_t* init;
     int* n18;
+    bool reset;
+    int kind, check;
   };
-  std::vector<ResetEntry> reset_list;
+  std::vector<StateEntry> state_list;
+  StreamStateTable state_table{};    // the list as the record kernels see it (built at the end of create)
+  uint64_t model_fingerprint = 0;    // of the loaded weights (ModelFingerprint), part of every record header
+  uint32_t* d_records = nullptr;     // export / import staging: records_chunk records (allocated on first use)
+  int records_chunk = 0;
   uint8_t* d_blob = nullptr;
   // streaming state, one block per kernel
   uint32_t* d_state[4] = {nullptr, nullptr, nullptr, nullptr};
@@ -78,7 +88,7 @@ struct lyra_b200_ctx {
   // decoder packet-loss path (PlcPlanKernel / ComfortNoiseKernel / PlcMixKernel)
   int* d_plc = nullptr;                      // [max_streams][4] concealment_progress, fade_progress, fade_direction, -
   double* d_cng_work = nullptr;              // [max_streams][1024] overlap-add buffers of the comfort-noise generators
-  unsigned long long* d_cng_hops = nullptr;  // [max_streams]
+  unsigned long long* d_cng_hops = nullptr;  // [max_streams][2] {hop counter, comfort-noise key offset} (ComfortNoiseKernel)
   unsigned long long cng_seed = 0;
   uint8_t* d_plan = nullptr;                 // by slot
   uint8_t* d_skip = nullptr;
@@ -622,12 +632,14 @@ std::vector<uint32_t> InitImage(const ModelSpec& s, int which) {
   return v;
 }
 
-// lyra_b200_reset: every entry of ctx->reset_list, for the listed streams (repeats are harmless), in order on ctx->stream
+// lyra_b200_reset: every entry of ctx->state_list that reset restores, for the listed streams (repeats are harmless), in order
+// on ctx->stream
 int ResetImpl(lyra_b200_ctx* ctx, const int32_t* ids, int n) {
   const int* d_ids = nullptr;
   int rc = CheckIds(ctx, ids, n, true);
   if (rc || (rc = UploadIds(ctx, ids, n, &d_ids))) return rc;
-  for (const lyra_b200_ctx::ResetEntry& e : ctx->reset_list) {
+  for (const lyra_b200_ctx::StateEntry& e : ctx->state_list) {
+    if (!e.reset) continue;
     LYRA_LAUNCH(ResetStateKernel, dim3((unsigned)n), dim3(256), (size_t)0, ctx->stream, e.state, e.init, e.words, e.lanes, d_ids, n, e.n18);
     ctx->launches += 1;
   }
@@ -645,12 +657,48 @@ bool DevAlloc(lyra_b200_ctx* ctx, T** p, size_t count) {
   return cudaMemset(*p, 0, bytes) == cudaSuccess;
 }
 
-// a device allocation of `per_stream` elements for each of the context's streams (row-major [padded][per_stream]) whose rows
-// lyra_b200_reset restores: to zero, or to the 4-byte words of `init` (a device image of one row)
+// a device allocation of `per_stream` elements for each of the context's streams (row-major [padded][per_stream]), listed in
+// ctx->state_list: lyra_b200_reset restores its rows (unless `reset` is false) to zero, or to the 4-byte words of `init` (a
+// device image of one row); the stream-state records carry them
 template <typename T>
-bool DevStreamState(lyra_b200_ctx* ctx, T** p, size_t per_stream, const uint32_t* init = nullptr) {
+bool DevStreamState(lyra_b200_ctx* ctx, T** p, size_t per_stream, const uint32_t* init = nullptr, int kind = kStatePlain,
+                    int check = lyra_b200_ctx::kCheckNone, bool reset = true) {
   if (!DevAlloc(ctx, p, (size_t)ctx->padded * per_stream)) return false;
-  ctx->reset_list.push_back({reinterpret_cast<uint32_t*>(*p), (int)(sizeof(T) * per_stream / 4), 1, init, nullptr});
+  ctx->state_list.push_back({reinterpret_cast<uint32_t*>(*p), (int)(sizeof(T) * per_stream / 4), 1, init, nullptr, reset, kind, check});
+  return true;
+}
+
+// 64-bit FNV-1a over the weight blob, 8 bytes at a time (and its size): tells records of another model apart
+uint64_t ModelFingerprint(const std::vector<uint8_t>& blob) {
+  uint64_t h = 0xcbf29ce484222325ull ^ (uint64_t)blob.size();
+  size_t i = 0;
+  for (; i + 8 <= blob.size(); i += 8) {
+    uint64_t w;
+    std::memcpy(&w, blob.data() + i, 8);
+    h = (h ^ w) * 0x100000001b3ull;
+  }
+  for (; i < blob.size(); ++i) h = (h ^ blob[i]) * 0x100000001b3ull;
+  return h;
+}
+
+// ctx->state_table from ctx->state_list (payload offsets in list order) and the constant header words
+bool BuildStateTable(lyra_b200_ctx* ctx) {
+  StreamStateTable& T = ctx->state_table;
+  if ((int)ctx->state_list.size() > kStateMaxEntries) return false;
+  int off = 0;
+  T.count = 0;
+  for (const lyra_b200_ctx::StateEntry& e : ctx->state_list) {
+    T.e[T.count++] = StreamStateEntry{e.state, e.init, e.n18, e.words, e.lanes, off, e.kind};
+    off += e.words + (e.n18 ? 1 : 0);
+  }
+  T.record_words = kStateHeaderWords + off;
+  std::memset(T.header, 0, sizeof(T.header));
+  T.header[kHdrMagic] = kStateMagic;
+  T.header[kHdrVersion] = kStateVersion;
+  T.header[kHdrBytes] = (uint32_t)(4 * T.record_words);
+  T.header[kHdrRoles] = (uint32_t)ctx->roles;
+  T.header[kHdrModelLo] = (uint32_t)ctx->model_fingerprint;
+  T.header[kHdrModelHi] = (uint32_t)(ctx->model_fingerprint >> 32);
   return true;
 }
 
@@ -713,6 +761,89 @@ int RunMaybeGraphed(lyra_b200_ctx* ctx, const lyra_b200_ctx::GraphKey& key, bool
 #endif
 }
 
+// ---- stream-state records (lyra_b200_export_streams / _import_streams / _copy_streams) ----
+
+size_t RecordBytes(const lyra_b200_ctx* ctx) { return 4 * (size_t)ctx->state_table.record_words; }
+
+// the export / import staging: as many records as fit in 64 MB (at least one, at most one kernel chunk), allocated on first use
+int EnsureRecordStaging(lyra_b200_ctx* ctx) {
+  if (ctx->d_records) return LYRA_B200_OK;
+  const size_t fit = ((size_t)64 << 20) / RecordBytes(ctx);
+  const int chunk = fit < 1 ? 1 : fit > (size_t)kStateChunk ? kStateChunk : (int)fit;
+  uint32_t* p = nullptr;
+  CU(cudaMalloc(reinterpret_cast<void**>(&p), RecordBytes(ctx) * (size_t)chunk));
+  ctx->allocs.push_back(p);
+  ctx->d_records = p;
+  ctx->records_chunk = chunk;
+  return LYRA_B200_OK;
+}
+
+uint32_t RecordWord(const uint8_t* rec, int i) {
+  uint32_t w;
+  std::memcpy(&w, rec + 4 * (size_t)i, 4);
+  return w;
+}
+
+// Why record `rec` cannot be imported into this context (nullptr: it can).  Besides the header, the payload words that index
+// memory are range-checked, so a damaged record cannot make a kernel read out of bounds: hop counters, the decoder control state
+// (as lyra_b200_plc_set_state) and the resamplers' positions.
+const char* RecordProblem(const lyra_b200_ctx* ctx, const uint8_t* rec) {
+  const StreamStateTable& T = ctx->state_table;
+  if (RecordWord(rec, kHdrMagic) != kStateMagic) return "not a stream-state record";
+  if (RecordWord(rec, kHdrVersion) != kStateVersion) return "record format version differs";
+  if (RecordWord(rec, kHdrBytes) != T.header[kHdrBytes] || RecordWord(rec, kHdrRoles) != T.header[kHdrRoles])
+    return "record size / roles differ from this context's";
+  if (RecordWord(rec, kHdrRate) != (uint32_t)ctx->sample_rate) return "record is from a context at another sample rate";
+  if (RecordWord(rec, kHdrModelLo) != T.header[kHdrModelLo] || RecordWord(rec, kHdrModelHi) != T.header[kHdrModelHi])
+    return "record is from another model";
+  if (RecordWord(rec, kHdrZero5) || RecordWord(rec, kHdrLive0) > 1 || RecordWord(rec, kHdrLive1) > 1) return "malformed record header";
+  for (int i = kHdrKeyHi + 1; i < kStateHeaderWords; ++i)
+    if (RecordWord(rec, i)) return "malformed record header";
+  for (int i = 0; i < T.count; ++i) {
+    const StreamStateEntry& e = T.e[i];
+    const int w0 = kStateHeaderWords + e.offset;
+    if (e.n18 && RecordWord(rec, w0 + e.words) >= 18u) return "hop counter out of range";
+    const int check = ctx->state_list[(size_t)i].check;
+    if (check == lyra_b200_ctx::kCheckResamplerPos && (int32_t)RecordWord(rec, w0) < 0) return "resampler position out of range";
+    if (check == lyra_b200_ctx::kCheckPlc) {
+      const int cp = (int32_t)RecordWord(rec, w0), fp = (int32_t)RecordWord(rec, w0 + 1), dir = (int32_t)RecordWord(rec, w0 + 2);
+      if (cp < 0 || cp > kPlcConcealSamples || cp % 320 || fp < 0 || fp > kPlcFadeSamples || fp % 320 || (dir != 1 && dir != -1))
+        return "decoder control state out of range";
+    }
+  }
+  return nullptr;
+}
+
+// ids for lyra_b200_copy_streams: n in [1, max_streams]; src in [-1, max_streams), dst in [0, max_streams); no repeats within
+// src (-1 excepted) or dst, no id in both
+int CheckCopyIds(lyra_b200_ctx* ctx, const int32_t* src, const int32_t* dst, int n) {
+  if (n <= 0 || n > ctx->max_streams) { ctx->err = "stream count out of range"; return LYRA_B200_EINVAL; }
+  uint32_t g[2];
+  for (uint32_t& x : g) {
+    if (++ctx->id_gen == 0) { std::fill(ctx->id_seen.begin(), ctx->id_seen.end(), 0u); ctx->id_gen = 1; }
+    x = ctx->id_gen;
+  }
+  for (int k = 0; k < n; ++k) {
+    const int id = src[k];
+    if (id < -1 || id >= ctx->max_streams) { ctx->err = "source stream id out of range"; return LYRA_B200_EINVAL; }
+    if (id < 0) continue;
+    if (ctx->id_seen[(size_t)id] == g[0]) { ctx->err = "repeated source stream id"; return LYRA_B200_EINVAL; }
+    ctx->id_seen[(size_t)id] = g[0];
+  }
+  for (int k = 0; k < n; ++k) {
+    const int id = dst[k];
+    if (id < 0 || id >= ctx->max_streams) { ctx->err = "destination stream id out of range"; return LYRA_B200_EINVAL; }
+    if (ctx->id_seen[(size_t)id] == g[1]) { ctx->err = "repeated destination stream id"; return LYRA_B200_EINVAL; }
+    if (ctx->id_seen[(size_t)id] == g[0]) { ctx->err = "a stream id is both a source and a destination"; return LYRA_B200_EINVAL; }
+    ctx->id_seen[(size_t)id] = g[1];
+  }
+  return LYRA_B200_OK;
+}
+
+// grid of a record kernel over `rows` rows of a call: 8 rows per block, one block row per state-list entry (+ `extra`)
+dim3 StateGrid(const lyra_b200_ctx* ctx, int rows, int extra) {
+  return dim3((unsigned)((rows + kStateRows - 1) / kStateRows), (unsigned)(ctx->state_table.count + extra));
+}
 
 }  // namespace
 
@@ -790,7 +921,7 @@ int lyra_b200_create_ex(const char* model_dir, int device, int max_streams, int 
     ok = ok && DevAlloc(ctx, &d_init, img.size());
     ok = ok && cudaMemcpy(d_init, img.data(), img.size() * 4, cudaMemcpyHostToDevice) == cudaSuccess;
     ok = ok && DevAlloc(ctx, &ctx->d_n18[w], P);
-    if (ok) ctx->reset_list.push_back({ctx->d_state[w], units[w], kTileStreams, d_init, ctx->d_n18[w]});
+    if (ok) ctx->state_list.push_back({ctx->d_state[w], units[w], kTileStreams, d_init, ctx->d_n18[w], true, kStatePlain, lyra_b200_ctx::kCheckNone});
   }
   if (roles & LYRA_B200_ROLE_ENCODER) ok = ok && DevAlloc(ctx, &ctx->d_mid_enc, P * 128 * 4);
   if (roles & LYRA_B200_ROLE_DECODER) ok = ok && DevAlloc(ctx, &ctx->d_mid_dec, P * 128 * 4);
@@ -808,9 +939,9 @@ int lyra_b200_create_ex(const char* model_dir, int device, int max_streams, int 
   uint32_t* d_plc0 = nullptr;
   ok = ok && DevAlloc(ctx, &d_plc0, 4);
   ok = ok && cudaMemcpy(d_plc0, plc0, sizeof(plc0), cudaMemcpyHostToDevice) == cudaSuccess;
-  ok = ok && DevStreamState(ctx, &ctx->d_plc, 4, d_plc0);
+  ok = ok && DevStreamState(ctx, &ctx->d_plc, 4, d_plc0, kStatePlain, lyra_b200_ctx::kCheckPlc);
   ok = ok && DevStreamState(ctx, &ctx->d_cng_work, 1024);
-  ok = ok && DevStreamState(ctx, &ctx->d_cng_hops, 1);
+  ok = ok && DevStreamState(ctx, &ctx->d_cng_hops, 2, nullptr, kStateCng);
   ok = ok && DevAlloc(ctx, &ctx->d_plan, P);
   ok = ok && DevAlloc(ctx, &ctx->d_skip, P);
   ok = ok && DevAlloc(ctx, &ctx->d_feed, P);
@@ -821,15 +952,17 @@ int lyra_b200_create_ex(const char* model_dir, int device, int max_streams, int 
   ok = ok && DevAlloc(ctx, &ctx->d_cng_pcm, P * LYRA_B200_HOP);
   ok = ok && DevAlloc(ctx, &ctx->d_cng_feat, P * 160);
   for (int d = 0; d < 2; ++d) {
-    // reset leaves the delay line alone: rate 0 in d_rs_pos makes the next call restart the stream fully primed
-    ok = ok && DevAlloc(ctx, &ctx->d_rs_delay[d], P * (size_t)(kResamplerTaps - 1));
-    ok = ok && DevStreamState(ctx, &ctx->d_rs_pos[d], 2);
+    // reset leaves the delay line alone: rate 0 in d_rs_pos makes the next call restart the stream fully primed (a stream
+    // moved mid-phase needs it, so the records carry it)
+    ok = ok && DevStreamState(ctx, &ctx->d_rs_delay[d], (size_t)(kResamplerTaps - 1), nullptr, kStatePlain, lyra_b200_ctx::kCheckNone, false);
+    ok = ok && DevStreamState(ctx, &ctx->d_rs_pos[d], 2, nullptr, kStatePlain, lyra_b200_ctx::kCheckResamplerPos);
   }
   for (int d = 0; d < 2; ++d) {
     // the codec path's converters (lyra_b200_set_sample_rate): reset zeroes them, and tag 0 makes the next call restart primed
     if (!(roles & (d == 0 ? LYRA_B200_ROLE_ENCODER : LYRA_B200_ROLE_DECODER))) continue;
     ok = ok && DevStreamState(ctx, &ctx->d_codec_rs_delay[d], (size_t)(kResamplerTaps - 1));
-    ok = ok && DevStreamState(ctx, &ctx->d_codec_rs_pos[d], 2);
+    ok = ok && DevStreamState(ctx, &ctx->d_codec_rs_pos[d], 2, nullptr, d == 0 ? kStateCodecRs0 : kStateCodecRs1,
+                              lyra_b200_ctx::kCheckResamplerPos);
   }
   ok = ok && DevAlloc(ctx, &ctx->d_rs_in, P * 960);
   ok = ok && DevAlloc(ctx, &ctx->d_rs_out, P * 968);
@@ -851,6 +984,8 @@ int lyra_b200_create_ex(const char* model_dir, int device, int max_streams, int 
     if (ok) for (size_t i = 0; i < P; ++i) ctx->h_slot_of[b][i] = -1;
   }
   if (ok) ok = SetSmemLimits();
+  ctx->model_fingerprint = ModelFingerprint(ctx->spec.blob);
+  ok = ok && BuildStateTable(ctx);
   if (!ok) {
     g_create_error = std::string("CUDA allocation / setup failed: ") + cudaGetErrorString(cudaGetLastError());
     lyra_b200_destroy(ctx);
@@ -1315,6 +1450,73 @@ int lyra_b200_resample(lyra_b200_ctx* ctx, int to_internal, const int32_t* ids, 
   CU(cudaMemcpyAsync(counts.data(), ctx->d_rs_counts, sizeof(int) * (size_t)n, cudaMemcpyDeviceToHost, ctx->stream));
   CU(SyncStream(ctx));
   if (out_counts) for (int k = 0; k < n; ++k) out_counts[k] = counts[(size_t)k];
+  return LYRA_B200_OK;
+}
+
+int lyra_b200_stream_state_bytes(const lyra_b200_ctx* ctx) { return ctx ? (int)RecordBytes(ctx) : 0; }
+
+int lyra_b200_export_streams(lyra_b200_ctx* ctx, const int32_t* stream_ids, int n, void* records) {
+  if (!ctx || !records) return LYRA_B200_EINVAL;
+  ENTER(0);
+  int rc = CheckIds(ctx, stream_ids, n, true);
+  if (rc || (rc = EnsureRecordStaging(ctx))) return rc;
+  ctx->state_table.header[kHdrRate] = (uint32_t)ctx->sample_rate;
+  const size_t rb = RecordBytes(ctx);
+  StreamIdChunk ids;
+  for (int k0 = 0; k0 < n; k0 += ctx->records_chunk) {
+    ids.n = n - k0 < ctx->records_chunk ? n - k0 : ctx->records_chunk;
+    for (int k = 0; k < ids.n; ++k) ids.src[k] = stream_ids ? stream_ids[k0 + k] : k0 + k;
+    LYRA_LAUNCH(StreamStateGatherKernel, StateGrid(ctx, ids.n, 1), dim3(kStateThreads), (size_t)kStateSmemBytes, ctx->stream,
+                ctx->state_table, ids, ctx->d_records, ctx->codec_rs_tag);
+    ctx->launches += 1;
+    CU(cudaGetLastError());
+    CU(cudaMemcpyAsync(static_cast<uint8_t*>(records) + rb * (size_t)k0, ctx->d_records, rb * (size_t)ids.n, cudaMemcpyDeviceToHost, ctx->stream));
+  }
+  CU(SyncStream(ctx));
+  return LYRA_B200_OK;
+}
+
+int lyra_b200_import_streams(lyra_b200_ctx* ctx, const int32_t* stream_ids, int n, const void* records) {
+  if (!ctx || !records) return LYRA_B200_EINVAL;
+  ENTER(0);
+  int rc = CheckIds(ctx, stream_ids, n, false);
+  if (rc) return rc;
+  const size_t rb = RecordBytes(ctx);
+  const uint8_t* recs = static_cast<const uint8_t*>(records);
+  for (int k = 0; k < n; ++k)                      // every record first: a bad one changes nothing
+    if (const char* why = RecordProblem(ctx, recs + rb * (size_t)k)) {
+      ctx->err = "record " + std::to_string(k) + ": " + why;
+      return LYRA_B200_EINVAL;
+    }
+  if ((rc = EnsureRecordStaging(ctx))) return rc;
+  StreamIdChunk ids;
+  for (int k0 = 0; k0 < n; k0 += ctx->records_chunk) {
+    ids.n = n - k0 < ctx->records_chunk ? n - k0 : ctx->records_chunk;
+    for (int k = 0; k < ids.n; ++k) ids.dst[k] = stream_ids ? stream_ids[k0 + k] : k0 + k;
+    CU(cudaMemcpyAsync(ctx->d_records, recs + rb * (size_t)k0, rb * (size_t)ids.n, cudaMemcpyHostToDevice, ctx->stream));
+    LYRA_LAUNCH(StreamStateScatterKernel, StateGrid(ctx, ids.n, 0), dim3(kStateThreads), (size_t)kStateSmemBytes, ctx->stream,
+                ctx->state_table, ids, ctx->d_records, ctx->codec_rs_tag);
+    ctx->launches += 1;
+    CU(cudaGetLastError());
+  }
+  CU(SyncStream(ctx));
+  return LYRA_B200_OK;
+}
+
+int lyra_b200_copy_streams(lyra_b200_ctx* ctx, const int32_t* src_ids, const int32_t* dst_ids, int n) {
+  if (!ctx || !src_ids || !dst_ids) return LYRA_B200_EINVAL;
+  ENTER(0);
+  const int rc = CheckCopyIds(ctx, src_ids, dst_ids, n);
+  if (rc) return rc;
+  StreamIdChunk ids;                               // the ids travel as kernel parameters: nothing to stage, nothing to wait for
+  for (int k0 = 0; k0 < n; k0 += kStateChunk) {
+    ids.n = n - k0 < kStateChunk ? n - k0 : kStateChunk;
+    std::memcpy(ids.src, src_ids + k0, sizeof(int) * (size_t)ids.n);
+    std::memcpy(ids.dst, dst_ids + k0, sizeof(int) * (size_t)ids.n);
+    LYRA_LAUNCH(StreamStateCopyKernel, StateGrid(ctx, ids.n, 0), dim3(kStateThreads), (size_t)0, ctx->stream, ctx->state_table, ids);
+    ctx->launches += 1;
+  }
+  CU(cudaGetLastError());
   return LYRA_B200_OK;
 }
 

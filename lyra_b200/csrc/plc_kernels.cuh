@@ -85,7 +85,8 @@ __device__ __forceinline__ void IfftStages3(double* re, double* im, int base, in
 // One block of 128 threads per stream.  features: [n][160] conditioning log-mel vectors (by slot), or nullptr = the stream's
 // current noise estimate (the first 160 floats of its noise-estimator state, LyraDecoder::RunComfortNoiseGenerator,
 // lyra/lyra_decoder.cc:328-340).  plan: nullptr = every slot runs; otherwise only slots with bit 2.
-// work: [max_streams][1024] f64 overlap-add buffers; hops: [max_streams] hop counters (phase draw).
+// work: [max_streams][1024] f64 overlap-add buffers; hops: [max_streams][2] {hop counter, key offset}: the phases of stream s are
+// drawn from key seed + s + offset (offset 0 unless the stream's state was moved here by lyra_b200_import_streams / _copy_streams).
 constexpr int kCngThreads = 128;
 __global__ void __launch_bounds__(kCngThreads)
 ComfortNoiseKernel(const uint8_t* __restrict__ blob, CngParams P, const int* __restrict__ stream_ids, int n,
@@ -110,8 +111,8 @@ ComfortNoiseKernel(const uint8_t* __restrict__ blob, CngParams P, const int* __r
   const double* synth = BlobPtr<double>(blob, P.synth);
   const double2* tw = BlobPtr<double2>(blob, P.twiddle);
   const float* f = features ? features + (size_t)slot * P.num_mel : noise_state + (size_t)stream * noise_units;
-  const unsigned long long hop_index = hops[stream];
-  const unsigned long long sseed = seed + (unsigned long long)stream;
+  const unsigned long long hop_index = hops[2 * (size_t)stream];
+  const unsigned long long sseed = seed + (unsigned long long)stream + hops[2 * (size_t)stream + 1];
   // mel[c] = (double)(float)exp(feature * 10)   (FftFromFeatures, .cc:87-96; exp of a float evaluated in double, rounded once)
   for (int c = tid; c < P.num_mel; c += NT) mel[c] = (double)(float)exp((double)__fmul_rn(f[c], 10.0f));
   for (int i = tid; i < N; i += NT) { xr0[FftIdx(i)] = 0.0; xi0[FftIdx(i)] = 0.0; }
@@ -174,7 +175,7 @@ ComfortNoiseKernel(const uint8_t* __restrict__ blob, CngParams P, const int* __r
     v = v < 32767.0 ? v : 32767.0;
     out[(size_t)slot * P.hop + i] = (int16_t)v;
   }
-  if (tid == 0) hops[stream] = hop_index + 1;
+  if (tid == 0) hops[2 * (size_t)stream] = hop_index + 1;
 }
 
 // out = model hop, comfort-noise hop, or their raised-cosine cross-fade (lyra_decoder.cc:342-373); 320 threads per slot
