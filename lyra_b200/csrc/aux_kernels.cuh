@@ -1,4 +1,4 @@
-// RVQ encode/decode + bit packing, state reset and the log-mel front end.
+// RVQ encode/decode + bit packing, per-stream state records and the log-mel front end.
 #pragma once
 
 #include "kernel_prims.cuh"
@@ -112,26 +112,9 @@ RvqDecodeKernel(const uint8_t* __restrict__ blob, RvqParams P, const uint8_t* __
 }
 
 // ------------------------------------------------------------------------------------------------
-// Reset the streaming state of selected streams to the reference's CALL_ONCE initial values
-// (all-zero resource variables; int8 rings hold the zero point of their tensor).  state[tile][unit][S] with
-// tile = stream / S, lane = stream % S; S = 1 is a row-major [stream][units] buffer.  init == nullptr: all zero;
-// n18 == nullptr: the state has no hop counter.
-__global__ void __launch_bounds__(256)
-ResetStateKernel(uint32_t* __restrict__ state, const uint32_t* __restrict__ init, int units, int S,
-                 const int* __restrict__ streams, int nstreams, int* __restrict__ n18) {
-  const int k = (int)blockIdx.x;
-  if (k >= nstreams) return;
-  const int stream = streams ? streams[k] : k;
-  const int tile = stream / S, lane = stream % S;
-  uint32_t* st = state + (size_t)tile * units * S + lane;
-  for (int u = (int)threadIdx.x; u < units; u += (int)blockDim.x) st[(size_t)u * S] = init ? init[u] : 0u;
-  if (n18 && threadIdx.x == 0) n18[stream] = 0;
-}
-
-// ------------------------------------------------------------------------------------------------
-// Per-stream state records: lyra_b200_export_streams (gather), _import_streams (scatter), _copy_streams (copy).  Every kernel is
-// one launch over all entries of the context's state list (blockIdx.y = entry) and 8 consecutive rows of the call per block
-// (blockIdx.x).  A tile-blocked entry (lanes = 8) is read / written with the 8 rows of a block on 8 consecutive threads, so rows
+// Per-stream state records: lyra_b200_export_streams (gather), _import_streams (scatter), _copy_streams and _reset (copy).
+// Every kernel is one launch over all entries of a state table (blockIdx.y = entry; reset's table leaves out the entries reset
+// keeps) and 8 consecutive rows of the call per block (blockIdx.x).  A tile-blocked entry (lanes = 8) is read / written with the 8 rows of a block on 8 consecutive threads, so rows
 // that are the 8 lanes of one tile move whole 32-byte tile rows; the records side goes through shared memory and moves whole
 // lines.  Row-major entries (lanes = 1) are contiguous per stream on both sides.
 //

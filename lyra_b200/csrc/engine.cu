@@ -54,21 +54,19 @@ struct lyra_b200_ctx {
   int roles = LYRA_B200_ROLE_ENCODER | LYRA_B200_ROLE_DECODER;   // which halves of the streaming state this context holds
   std::vector<void*> allocs;         // every device allocation of the context (lyra_b200_destroy frees them)
   // Every piece of per-stream state, in one list that drives lyra_b200_reset, _export_streams, _import_streams and
-  // _copy_streams: `words` 4-byte words per stream at lane stride `lanes` (layout of ResetStateKernel), initial image `init`
+  // _copy_streams: `words` 4-byte words per stream at lane stride `lanes` (layout of StateWord), initial image `init`
   // (nullptr: zero), hop counter `n18` (nullptr: none; initially 0).  `reset` = false: lyra_b200_reset leaves the entry alone
   // (lyra_b200_resample's delay lines).  `kind` (StreamStateKind) marks the words a record does not carry verbatim; `check`
   // is what import validates in a record's payload besides the hop counter.
   enum Check { kCheckNone, kCheckPlc, kCheckResamplerPos };
   struct StateEntry {
-    uint32_t* state;
-    int words, lanes;
-    const uint32_t* init;
-    int* n18;
+    StreamStateEntry e;              // e.offset is set by BuildStateTable
     bool reset;
-    int kind, check;
+    int check;
   };
   std::vector<StateEntry> state_list;
   StreamStateTable state_table{};    // the list as the record kernels see it (built at the end of create)
+  StreamStateTable reset_table{};    // its entries that lyra_b200_reset restores
   uint64_t model_fingerprint = 0;    // of the loaded weights (ModelFingerprint), part of every record header
   uint32_t* d_records = nullptr;     // export / import staging: records_chunk records (allocated on first use)
   int records_chunk = 0;
@@ -253,17 +251,23 @@ bool BitsOk(lyra_b200_ctx* ctx, int num_bits) {
   return true;
 }
 
+// A fresh stamp for ctx->id_seen: no stream is marked with it yet
+uint32_t NextIdGen(lyra_b200_ctx* ctx) {
+  if (++ctx->id_gen == 0) { std::fill(ctx->id_seen.begin(), ctx->id_seen.end(), 0u); ctx->id_gen = 1; }
+  return ctx->id_gen;
+}
+
 // The rows of a call: n in [1, max_streams]; ids (nullptr: streams 0..n-1) in range and, unless allow_repeats, distinct.
 int CheckIds(lyra_b200_ctx* ctx, const int32_t* ids, int n, bool allow_repeats) {
   if (n <= 0 || n > ctx->max_streams) { ctx->err = "stream count out of range"; return LYRA_B200_EINVAL; }
   if (!ids) return LYRA_B200_OK;
-  if (++ctx->id_gen == 0) { std::fill(ctx->id_seen.begin(), ctx->id_seen.end(), 0u); ctx->id_gen = 1; }
+  const uint32_t gen = NextIdGen(ctx);
   for (int k = 0; k < n; ++k) {
     const int id = ids[k];
     if (id < 0 || id >= ctx->max_streams) { ctx->err = "stream id out of range"; return LYRA_B200_EINVAL; }
     if (allow_repeats) continue;
-    if (ctx->id_seen[(size_t)id] == ctx->id_gen) { ctx->err = "duplicate stream id in one call"; return LYRA_B200_EINVAL; }
-    ctx->id_seen[(size_t)id] = ctx->id_gen;
+    if (ctx->id_seen[(size_t)id] == gen) { ctx->err = "duplicate stream id in one call"; return LYRA_B200_EINVAL; }
+    ctx->id_seen[(size_t)id] = gen;
   }
   return LYRA_B200_OK;
 }
@@ -632,22 +636,6 @@ std::vector<uint32_t> InitImage(const ModelSpec& s, int which) {
   return v;
 }
 
-// lyra_b200_reset: every entry of ctx->state_list that reset restores, for the listed streams (repeats are harmless), in order
-// on ctx->stream
-int ResetImpl(lyra_b200_ctx* ctx, const int32_t* ids, int n) {
-  const int* d_ids = nullptr;
-  int rc = CheckIds(ctx, ids, n, true);
-  if (rc || (rc = UploadIds(ctx, ids, n, &d_ids))) return rc;
-  for (const lyra_b200_ctx::StateEntry& e : ctx->state_list) {
-    if (!e.reset) continue;
-    LYRA_LAUNCH(ResetStateKernel, dim3((unsigned)n), dim3(256), (size_t)0, ctx->stream, e.state, e.init, e.words, e.lanes, d_ids, n, e.n18);
-    ctx->launches += 1;
-  }
-  CU(cudaGetLastError());
-  CU(SyncStream(ctx));
-  return LYRA_B200_OK;
-}
-
 // a zero-filled device allocation of `count` elements, recorded in ctx->allocs
 template <typename T>
 bool DevAlloc(lyra_b200_ctx* ctx, T** p, size_t count) {
@@ -657,14 +645,20 @@ bool DevAlloc(lyra_b200_ctx* ctx, T** p, size_t count) {
   return cudaMemset(*p, 0, bytes) == cudaSuccess;
 }
 
-// a device allocation of `per_stream` elements for each of the context's streams (row-major [padded][per_stream]), listed in
-// ctx->state_list: lyra_b200_reset restores its rows (unless `reset` is false) to zero, or to the 4-byte words of `init` (a
-// device image of one row); the stream-state records carry them
+// a device allocation of `per_stream` elements for each of the context's streams at lane stride `lanes` (1: row-major
+// [padded][per_stream]; 8: [tile][per_stream][8]), and with n18 != nullptr a hop counter per stream in *n18, appended to
+// ctx->state_list with a device copy of `init` (host image of one row; nullptr: zero).  lyra_b200_ctx::StateEntry says what
+// the other arguments mean.
 template <typename T>
-bool DevStreamState(lyra_b200_ctx* ctx, T** p, size_t per_stream, const uint32_t* init = nullptr, int kind = kStatePlain,
-                    int check = lyra_b200_ctx::kCheckNone, bool reset = true) {
+bool DevStreamState(lyra_b200_ctx* ctx, T** p, size_t per_stream, const void* init = nullptr, int kind = kStatePlain,
+                    int check = lyra_b200_ctx::kCheckNone, bool reset = true, int lanes = 1, int** n18 = nullptr) {
+  const int words = (int)(sizeof(T) * per_stream / 4);
+  uint32_t* d_init = nullptr;
   if (!DevAlloc(ctx, p, (size_t)ctx->padded * per_stream)) return false;
-  ctx->state_list.push_back({reinterpret_cast<uint32_t*>(*p), (int)(sizeof(T) * per_stream / 4), 1, init, nullptr, reset, kind, check});
+  if (n18 && !DevAlloc(ctx, n18, (size_t)ctx->padded)) return false;
+  if (init && !(DevAlloc(ctx, &d_init, (size_t)words) && cudaMemcpy(d_init, init, 4 * (size_t)words, cudaMemcpyHostToDevice) == cudaSuccess))
+    return false;
+  ctx->state_list.push_back({{reinterpret_cast<uint32_t*>(*p), d_init, n18 ? *n18 : nullptr, words, lanes, 0, kind}, reset, check});
   return true;
 }
 
@@ -681,15 +675,18 @@ uint64_t ModelFingerprint(const std::vector<uint8_t>& blob) {
   return h;
 }
 
-// ctx->state_table from ctx->state_list (payload offsets in list order) and the constant header words
+// ctx->state_table from ctx->state_list (payload offsets in list order) and the constant header words; ctx->reset_table
 bool BuildStateTable(lyra_b200_ctx* ctx) {
   StreamStateTable& T = ctx->state_table;
+  StreamStateTable& R = ctx->reset_table;
   if ((int)ctx->state_list.size() > kStateMaxEntries) return false;
   int off = 0;
-  T.count = 0;
-  for (const lyra_b200_ctx::StateEntry& e : ctx->state_list) {
-    T.e[T.count++] = StreamStateEntry{e.state, e.init, e.n18, e.words, e.lanes, off, e.kind};
-    off += e.words + (e.n18 ? 1 : 0);
+  T.count = R.count = 0;
+  for (lyra_b200_ctx::StateEntry& s : ctx->state_list) {
+    s.e.offset = off;
+    off += s.e.words + (s.e.n18 ? 1 : 0);
+    T.e[T.count++] = s.e;
+    if (s.reset) R.e[R.count++] = s.e;
   }
   T.record_words = kStateHeaderWords + off;
   std::memset(T.header, 0, sizeof(T.header));
@@ -778,6 +775,12 @@ int EnsureRecordStaging(lyra_b200_ctx* ctx) {
   return LYRA_B200_OK;
 }
 
+// a decoder control state lyra_b200_plc_set_state and import accept: hop-aligned concealment 0..1280, fade 0..640, direction +-1
+bool PlcStateOk(int cp, int fp, int dir) {
+  return cp >= 0 && cp <= kPlcConcealSamples && cp % 320 == 0 && fp >= 0 && fp <= kPlcFadeSamples && fp % 320 == 0 &&
+         (dir == 1 || dir == -1);
+}
+
 uint32_t RecordWord(const uint8_t* rec, int i) {
   uint32_t w;
   std::memcpy(&w, rec + 4 * (size_t)i, 4);
@@ -805,11 +808,9 @@ const char* RecordProblem(const lyra_b200_ctx* ctx, const uint8_t* rec) {
     if (e.n18 && RecordWord(rec, w0 + e.words) >= 18u) return "hop counter out of range";
     const int check = ctx->state_list[(size_t)i].check;
     if (check == lyra_b200_ctx::kCheckResamplerPos && (int32_t)RecordWord(rec, w0) < 0) return "resampler position out of range";
-    if (check == lyra_b200_ctx::kCheckPlc) {
-      const int cp = (int32_t)RecordWord(rec, w0), fp = (int32_t)RecordWord(rec, w0 + 1), dir = (int32_t)RecordWord(rec, w0 + 2);
-      if (cp < 0 || cp > kPlcConcealSamples || cp % 320 || fp < 0 || fp > kPlcFadeSamples || fp % 320 || (dir != 1 && dir != -1))
-        return "decoder control state out of range";
-    }
+    if (check == lyra_b200_ctx::kCheckPlc &&
+        !PlcStateOk((int32_t)RecordWord(rec, w0), (int32_t)RecordWord(rec, w0 + 1), (int32_t)RecordWord(rec, w0 + 2)))
+      return "decoder control state out of range";
   }
   return nullptr;
 }
@@ -818,11 +819,7 @@ const char* RecordProblem(const lyra_b200_ctx* ctx, const uint8_t* rec) {
 // src (-1 excepted) or dst, no id in both
 int CheckCopyIds(lyra_b200_ctx* ctx, const int32_t* src, const int32_t* dst, int n) {
   if (n <= 0 || n > ctx->max_streams) { ctx->err = "stream count out of range"; return LYRA_B200_EINVAL; }
-  uint32_t g[2];
-  for (uint32_t& x : g) {
-    if (++ctx->id_gen == 0) { std::fill(ctx->id_seen.begin(), ctx->id_seen.end(), 0u); ctx->id_gen = 1; }
-    x = ctx->id_gen;
-  }
+  const uint32_t g[2] = {NextIdGen(ctx), NextIdGen(ctx)};
   for (int k = 0; k < n; ++k) {
     const int id = src[k];
     if (id < -1 || id >= ctx->max_streams) { ctx->err = "source stream id out of range"; return LYRA_B200_EINVAL; }
@@ -840,9 +837,26 @@ int CheckCopyIds(lyra_b200_ctx* ctx, const int32_t* src, const int32_t* dst, int
   return LYRA_B200_OK;
 }
 
-// grid of a record kernel over `rows` rows of a call: 8 rows per block, one block row per state-list entry (+ `extra`)
-dim3 StateGrid(const lyra_b200_ctx* ctx, int rows, int extra) {
-  return dim3((unsigned)((rows + kStateRows - 1) / kStateRows), (unsigned)(ctx->state_table.count + extra));
+// grid of a record kernel over `rows` rows of a call: 8 rows per block, one block row per entry of T (+ `extra`)
+dim3 StateGrid(const StreamStateTable& T, int rows, int extra) {
+  return dim3((unsigned)((rows + kStateRows - 1) / kStateRows), (unsigned)(T.count + extra));
+}
+
+// StreamStateCopyKernel over the entries of T on ctx->stream, one launch per kStateChunk rows: stream dst[k] (nullptr: k) <-
+// stream src[k] (nullptr: -1, the state at creation).  The ids travel as kernel parameters: nothing to stage, nothing to wait for.
+int CopyStreamState(lyra_b200_ctx* ctx, const StreamStateTable& T, const int32_t* src, const int32_t* dst, int n) {
+  StreamIdChunk ids;
+  for (int k0 = 0; k0 < n; k0 += kStateChunk) {
+    ids.n = n - k0 < kStateChunk ? n - k0 : kStateChunk;
+    for (int k = 0; k < ids.n; ++k) {
+      ids.src[k] = src ? src[k0 + k] : -1;
+      ids.dst[k] = dst ? dst[k0 + k] : k0 + k;
+    }
+    LYRA_LAUNCH(StreamStateCopyKernel, StateGrid(T, ids.n, 0), dim3(kStateThreads), (size_t)0, ctx->stream, T, ids);
+    ctx->launches += 1;
+  }
+  CU(cudaGetLastError());
+  return LYRA_B200_OK;
 }
 
 }  // namespace
@@ -911,17 +925,12 @@ int lyra_b200_create_ex(const char* model_dir, int device, int max_streams, int 
   ctx->stream = ctx->own_stream;
   ok = ok && DevAlloc(ctx, &ctx->d_blob, ctx->spec.blob.size());
   ok = ok && cudaMemcpy(ctx->d_blob, ctx->spec.blob.data(), ctx->spec.blob.size(), cudaMemcpyHostToDevice) == cudaSuccess;
-  // Device memory.  DevStreamState allocates per-stream state and lists it for lyra_b200_reset; DevAlloc is everything else.
+  // Device memory.  DevStreamState allocates per-stream state and lists it in ctx->state_list; DevAlloc is everything else.
   const int units[4] = {EncStateA::kUnits, EncStateB::kUnits, DecStateC::kUnits, DecStateD::kUnits};
   for (int w = 0; w < 4 && ok; ++w) {
     if (!(roles & (w < 2 ? LYRA_B200_ROLE_ENCODER : LYRA_B200_ROLE_DECODER))) continue;   // an encoder-only / decoder-only context
-    const std::vector<uint32_t> img = InitImage(ctx->spec, w);
-    uint32_t* d_init = nullptr;
-    ok = ok && DevAlloc(ctx, &ctx->d_state[w], (size_t)units[w] * P);   // [tile][unit][kTileStreams]
-    ok = ok && DevAlloc(ctx, &d_init, img.size());
-    ok = ok && cudaMemcpy(d_init, img.data(), img.size() * 4, cudaMemcpyHostToDevice) == cudaSuccess;
-    ok = ok && DevAlloc(ctx, &ctx->d_n18[w], P);
-    if (ok) ctx->state_list.push_back({ctx->d_state[w], units[w], kTileStreams, d_init, ctx->d_n18[w], true, kStatePlain, lyra_b200_ctx::kCheckNone});
+    ok = DevStreamState(ctx, &ctx->d_state[w], (size_t)units[w], InitImage(ctx->spec, w).data(), kStatePlain, lyra_b200_ctx::kCheckNone,
+                        true, kTileStreams, &ctx->d_n18[w]);
   }
   if (roles & LYRA_B200_ROLE_ENCODER) ok = ok && DevAlloc(ctx, &ctx->d_mid_enc, P * 128 * 4);
   if (roles & LYRA_B200_ROLE_DECODER) ok = ok && DevAlloc(ctx, &ctx->d_mid_dec, P * 128 * 4);
@@ -936,10 +945,7 @@ int lyra_b200_create_ex(const char* model_dir, int device, int max_streams, int 
   ok = ok && DevStreamState(ctx, &ctx->d_logmel_prev_enc, LYRA_B200_HOP);
   // decoder control state: (0, 0, fade from comfort noise), lyra_decoder.cc:164-166
   const int plc0[4] = {0, 0, -1, 0};
-  uint32_t* d_plc0 = nullptr;
-  ok = ok && DevAlloc(ctx, &d_plc0, 4);
-  ok = ok && cudaMemcpy(d_plc0, plc0, sizeof(plc0), cudaMemcpyHostToDevice) == cudaSuccess;
-  ok = ok && DevStreamState(ctx, &ctx->d_plc, 4, d_plc0, kStatePlain, lyra_b200_ctx::kCheckPlc);
+  ok = ok && DevStreamState(ctx, &ctx->d_plc, 4, plc0, kStatePlain, lyra_b200_ctx::kCheckPlc);
   ok = ok && DevStreamState(ctx, &ctx->d_cng_work, 1024);
   ok = ok && DevStreamState(ctx, &ctx->d_cng_hops, 2, nullptr, kStateCng);
   ok = ok && DevAlloc(ctx, &ctx->d_plan, P);
@@ -991,7 +997,7 @@ int lyra_b200_create_ex(const char* model_dir, int device, int max_streams, int 
     lyra_b200_destroy(ctx);
     return LYRA_B200_ENODEV;
   }
-  if (ResetImpl(ctx, nullptr, max_streams) != LYRA_B200_OK) {
+  if (lyra_b200_reset(ctx, nullptr, max_streams) != LYRA_B200_OK) {
     g_create_error = ctx->err;
     lyra_b200_destroy(ctx);
     return LYRA_B200_ENODEV;
@@ -1048,10 +1054,24 @@ int lyra_b200_profile_read(lyra_b200_ctx* ctx, double* ms_sum, uint64_t* launche
   return LYRA_B200_OK;
 }
 
+// the entries of ctx->reset_table go back to their state at creation, in order on ctx->stream.  Repeated ids are collapsed
+// (first appearance kept): the copy kernel's destinations must be distinct.
 int lyra_b200_reset(lyra_b200_ctx* ctx, const int32_t* stream_ids, int n) {
   if (!ctx) return LYRA_B200_EINVAL;
   ENTER(0);
-  return ResetImpl(ctx, stream_ids, n);
+  int rc = CheckIds(ctx, stream_ids, n, true);
+  if (rc) return rc;
+  std::vector<int32_t> distinct;
+  if (stream_ids) {
+    const uint32_t gen = NextIdGen(ctx);
+    for (int k = 0; k < n; ++k)
+      if (ctx->id_seen[(size_t)stream_ids[k]] != gen) { ctx->id_seen[(size_t)stream_ids[k]] = gen; distinct.push_back(stream_ids[k]); }
+    stream_ids = distinct.data();
+    n = (int)distinct.size();
+  }
+  if ((rc = CopyStreamState(ctx, ctx->reset_table, nullptr, stream_ids, n))) return rc;
+  CU(SyncStream(ctx));
+  return LYRA_B200_OK;
 }
 
 int lyra_b200_set_stream(lyra_b200_ctx* ctx, void* cuda_stream) {
@@ -1393,7 +1413,7 @@ int lyra_b200_plc_set_state(lyra_b200_ctx* ctx, const int32_t* ids, int n, const
   for (int k = 0; k < n; ++k) {
     const int id = ids ? ids[k] : k;
     const int32_t* s3 = state + (size_t)k * 3;
-    if (s3[0] < 0 || s3[0] > kPlcConcealSamples || s3[0] % 320 || s3[1] < 0 || s3[1] > kPlcFadeSamples || s3[1] % 320 || (s3[2] != 1 && s3[2] != -1)) {
+    if (!PlcStateOk(s3[0], s3[1], s3[2])) {
       ctx->err = "decoder control state must be hop aligned: concealment 0..1280, fade 0..640, direction +-1";
       return LYRA_B200_EINVAL;
     }
@@ -1466,7 +1486,7 @@ int lyra_b200_export_streams(lyra_b200_ctx* ctx, const int32_t* stream_ids, int 
   for (int k0 = 0; k0 < n; k0 += ctx->records_chunk) {
     ids.n = n - k0 < ctx->records_chunk ? n - k0 : ctx->records_chunk;
     for (int k = 0; k < ids.n; ++k) ids.src[k] = stream_ids ? stream_ids[k0 + k] : k0 + k;
-    LYRA_LAUNCH(StreamStateGatherKernel, StateGrid(ctx, ids.n, 1), dim3(kStateThreads), (size_t)kStateSmemBytes, ctx->stream,
+    LYRA_LAUNCH(StreamStateGatherKernel, StateGrid(ctx->state_table, ids.n, 1), dim3(kStateThreads), (size_t)kStateSmemBytes, ctx->stream,
                 ctx->state_table, ids, ctx->d_records, ctx->codec_rs_tag);
     ctx->launches += 1;
     CU(cudaGetLastError());
@@ -1494,7 +1514,7 @@ int lyra_b200_import_streams(lyra_b200_ctx* ctx, const int32_t* stream_ids, int 
     ids.n = n - k0 < ctx->records_chunk ? n - k0 : ctx->records_chunk;
     for (int k = 0; k < ids.n; ++k) ids.dst[k] = stream_ids ? stream_ids[k0 + k] : k0 + k;
     CU(cudaMemcpyAsync(ctx->d_records, recs + rb * (size_t)k0, rb * (size_t)ids.n, cudaMemcpyHostToDevice, ctx->stream));
-    LYRA_LAUNCH(StreamStateScatterKernel, StateGrid(ctx, ids.n, 0), dim3(kStateThreads), (size_t)kStateSmemBytes, ctx->stream,
+    LYRA_LAUNCH(StreamStateScatterKernel, StateGrid(ctx->state_table, ids.n, 0), dim3(kStateThreads), (size_t)kStateSmemBytes, ctx->stream,
                 ctx->state_table, ids, ctx->d_records, ctx->codec_rs_tag);
     ctx->launches += 1;
     CU(cudaGetLastError());
@@ -1507,17 +1527,7 @@ int lyra_b200_copy_streams(lyra_b200_ctx* ctx, const int32_t* src_ids, const int
   if (!ctx || !src_ids || !dst_ids) return LYRA_B200_EINVAL;
   ENTER(0);
   const int rc = CheckCopyIds(ctx, src_ids, dst_ids, n);
-  if (rc) return rc;
-  StreamIdChunk ids;                               // the ids travel as kernel parameters: nothing to stage, nothing to wait for
-  for (int k0 = 0; k0 < n; k0 += kStateChunk) {
-    ids.n = n - k0 < kStateChunk ? n - k0 : kStateChunk;
-    std::memcpy(ids.src, src_ids + k0, sizeof(int) * (size_t)ids.n);
-    std::memcpy(ids.dst, dst_ids + k0, sizeof(int) * (size_t)ids.n);
-    LYRA_LAUNCH(StreamStateCopyKernel, StateGrid(ctx, ids.n, 0), dim3(kStateThreads), (size_t)0, ctx->stream, ctx->state_table, ids);
-    ctx->launches += 1;
-  }
-  CU(cudaGetLastError());
-  return LYRA_B200_OK;
+  return rc ? rc : CopyStreamState(ctx, ctx->state_table, src_ids, dst_ids, n);
 }
 
 int lyra_b200_noise_estimate(lyra_b200_ctx* ctx, const int32_t* ids, int n, float* noise_estimate, uint8_t* is_noise) {

@@ -205,10 +205,11 @@ def _every_stateful_call(ctx, f, ids, wav, bits):
 
 
 def run_reset_restores_every_stream_state(Context, api, wav, *, max_streams=16, ids=(1, 6, 9, 14), reset_ids=(9, 1, 9), dense_n=8,
-                                          hops=9, bits=64, cng_seed=3):
+                                          hops=9, bits=64, cng_seed=3, dense_launches=None):
     """lyra_b200_reset restores all per-stream state: three contexts run the same history through every stateful call, then one
     resets `reset_ids` (an id listed twice) and one resets streams 0..dense_n-1.  On the next hop a reset stream must equal a fresh
-    context's first hop and every other stream the twin that was not reset, in every output and in the control state, bit for bit."""
+    context's first hop and every other stream the twin that was not reset, in every output and in the control state, bit for bit.
+    dense_launches: the kernel launches the dense reset must take (one per 1024 streams)."""
     ids = np.asarray(ids, dtype=np.int32)
 
     def make():
@@ -224,7 +225,10 @@ def run_reset_restores_every_stream_state(Context, api, wav, *, max_streams=16, 
         seen_dtx |= bool((o["dtx_bytes"] == 0).any())
     assert seen_cn and seen_dtx, "the history must reach comfort noise and DTX"
     sparse.reset(np.asarray(reset_ids, dtype=np.int32))
+    launches = dense.launch_count
     dense.reset(n=dense_n)
+    if dense_launches is not None:
+        assert dense.launch_count - launches == dense_launches, "reset(n=%d) took %d launches" % (dense_n, dense.launch_count - launches)
     fresh = make()
     twin_state = twin.plc_state(stream_ids=ids)
     want = {True: _every_stateful_call(fresh, hops, ids, wav, bits), False: _every_stateful_call(twin, hops, ids, wav, bits)}

@@ -135,6 +135,12 @@ def test_reset_restores_every_stream_state(gpu_api, sample1):
                                              reset_ids=(40, 9, 1, 9), dense_n=16)
 
 
+def test_reset_across_launch_chunks(gpu_api, sample1):
+    # reset launches one copy kernel per 1024 streams: ids on both sides of the chunk edges at 1024 and 2048
+    pc.run_reset_restores_every_stream_state(_capi.Context, gpu_api, sample1, max_streams=2112, ids=(5, 1030, 2050, 2100),
+                                             reset_ids=(2050, 5, 2050), dense_n=2060, dense_launches=3)
+
+
 def test_error_paths(gpu_api):
     pc.run_error_paths(_capi.Context, gpu_api, _capi.LyraB200Error)
 
