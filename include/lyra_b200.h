@@ -96,8 +96,9 @@ int lyra_b200_copy_streams(lyra_b200_ctx* ctx, const int32_t* src_ids, const int
 
 /* The external sample rate of the fused codec calls (LyraEncoder::Create / LyraDecoder::Create's sample_rate_hz,
  * lyra/lyra_config.h:56): 8000, 16000 (default), 32000 or 48000; any other rate returns LYRA_B200_EINVAL and leaves the setting
- * unchanged.  The reference fixes the rate per encoder / decoder object; here it holds for every stream of the context (one
- * context per rate).
+ * unchanged.  The reference fixes the rate per encoder / decoder object; here it is the context's rate: it sets the row length
+ * of the calls below and puts every stream at that rate.  Streams may then run at lower rates of their own
+ * (lyra_b200_set_stream_sample_rates), so one context serves 8, 16, 32 and 48 kHz calls side by side.
  *   Calls that follow it: lyra_b200_encode, _encode_dtx, _decode, _decode_track_noise, _decode_plc and their *_device twins.
  *   Their PCM rows hold sample_rate_hz / 50 samples (one 20 ms hop at the external rate): input of the encoders, output of the
  *   decoders.  Packets, masks, flags and packet_bytes do not change.  Internally the codec runs at 16 kHz: the encoder role
@@ -108,12 +109,29 @@ int lyra_b200_copy_streams(lyra_b200_ctx* ctx, const int32_t* src_ids, const int
  *   constants follow the rate) and fed the 16 kHz hop; the decoder-side estimator and comfort noise stay at 16 kHz.
  *   Calls that ignore it: the plugin-level 16 kHz components extract_features, quantize, dequantize, generate, logmel,
  *   noise_update, noise_estimate, cng_generate, and resample.
- * At 16000 nothing is converted.  Setting the current rate does nothing.  A change waits for the context's queued work and
- * drops captured graphs (like lyra_b200_set_priority).  Streams keep their codec state (networks, estimators, packet-loss
- * state); each stream's converters restart fully primed on its next call, like a fresh Resampler.  A caller that wants a
- * brand-new LyraEncoder / LyraDecoder also calls lyra_b200_reset. */
+ * At 16000 nothing is converted (unless a stream has a rate of its own).  Setting the current rate when no stream has a rate of
+ * its own does nothing.  A change waits for the context's queued work and drops captured graphs (like lyra_b200_set_priority).
+ * Every stream is at the new rate afterwards.  Streams keep their codec state (networks, estimators, packet-loss state); each
+ * stream whose rate changed restarts its converters fully primed on its next call, like a fresh Resampler.  A caller that wants
+ * a brand-new LyraEncoder / LyraDecoder also calls lyra_b200_reset. */
 int lyra_b200_set_sample_rate(lyra_b200_ctx* ctx, int sample_rate_hz);
 int lyra_b200_sample_rate(const lyra_b200_ctx* ctx);
+/* Per-stream rates, one LyraEncoder / LyraDecoder pair per call at its own rate: stream stream_ids[k] (NULL: streams 0..n-1)
+ * runs the fused calls at rates_hz[k], one of 8000, 16000, 32000, 48000 and at most the context's rate (its hop must fit in the
+ * row).  In every fused call and *_device twin a stream at rate r uses the first r / 50 samples of its row: the encoders ignore
+ * the rest, the decoders write it as 0.  The encoder-side DTX estimator follows the stream's rate; the decoder side stays at
+ * 16 kHz.  An unsupported rate, a rate above the context's or a repeated id returns LYRA_B200_EINVAL and changes nothing.
+ * Works in any context.  Asynchronous like lyra_b200_copy_streams: queued on the installed stream, no host synchronisation, so
+ * a server admits a call with copy_streams(-1 -> slot) followed by its rate without draining.  A stream whose rate changes keeps
+ * its codec state, and its converters restart fully primed on its next call; setting a stream to the rate it has changes
+ * nothing.  lyra_b200_reset and copy_streams from -1 put a stream back at the context's rate; copy, export and import carry a
+ * stream's rate with it (a record still holds the context's rate and import still refuses another one).
+ * The rates are read on the device, so changing them does not invalidate captured graphs; the first stream given a rate of its
+ * own at 16 kHz adds the converters' launches to the calls, which then capture graphs of their own (lyra_b200_set_graphs). */
+int lyra_b200_set_stream_sample_rates(lyra_b200_ctx* ctx, const int32_t* stream_ids, int n, const int32_t* rates_hz);
+/* rates_hz[k] = the rate stream stream_ids[k] (NULL: k) runs at; an id may be listed more than once.  Ordered on the installed
+ * stream behind the work queued there; returns when done. */
+int lyra_b200_stream_sample_rates(lyra_b200_ctx* ctx, const int32_t* stream_ids, int n, int32_t* rates_hz);
 
 /* LyraEncoder::Encode without DTX (lyra/lyra_encoder.cc:113-156) for n streams:
  * pcm[n][sample_rate / 50] -> packets[n][ceil(num_bits/8)] (pcm[n][320] at the default 16 kHz; lyra_b200_set_sample_rate).

@@ -78,6 +78,8 @@ class CApi:
             "lyra_b200_resample": (ci, [vp, ci, vp, ci, ci, vp, ci, vp, ci, vp]),
             "lyra_b200_set_sample_rate": (ci, [vp, ci]),
             "lyra_b200_sample_rate": (ci, [vp]),
+            "lyra_b200_set_stream_sample_rates": (ci, [vp, vp, ci, vp]),
+            "lyra_b200_stream_sample_rates": (ci, [vp, vp, ci, vp]),
             "lyra_b200_stream_state_bytes": (ci, [vp]),
             "lyra_b200_export_streams": (ci, [vp, vp, ci, vp]),
             "lyra_b200_import_streams": (ci, [vp, vp, ci, vp]),
@@ -99,7 +101,7 @@ class CApi:
                "lyra_b200_profile_read", "lyra_b200_noise_estimate", "lyra_b200_decode_plc", "lyra_b200_decode_plc_device",
                "lyra_b200_plc_get_state", "lyra_b200_plc_set_state", "lyra_b200_cng_generate", "lyra_b200_set_cng_seed",
                "lyra_b200_encode_dtx", "lyra_b200_encode_dtx_device", "lyra_b200_resample", "lyra_b200_set_sample_rate",
-               "lyra_b200_sample_rate", "lyra_b200_stream_state_bytes", "lyra_b200_export_streams", "lyra_b200_import_streams",
+               "lyra_b200_sample_rate", "lyra_b200_set_stream_sample_rates", "lyra_b200_stream_sample_rates", "lyra_b200_stream_state_bytes", "lyra_b200_export_streams", "lyra_b200_import_streams",
                "lyra_b200_copy_streams"]
 
 
@@ -217,6 +219,21 @@ class Context:
     @property
     def sample_rate(self):
         return int(self.api.lib.lyra_b200_sample_rate(self.h))
+
+    def set_stream_sample_rates(self, rates, stream_ids=None):
+        """Streams `stream_ids` (default: 0..len(rates)-1) run the fused calls at rates[k] (8000 / 16000 / 32000 / 48000, at most
+        sample_rate): they use the first rate // 50 samples of their rows.  Asynchronous on the installed stream."""
+        r = np.ascontiguousarray(rates, dtype=np.int32).reshape(-1)
+        ids = _ids(stream_ids, r.size)
+        self._check(self.api.lib.lyra_b200_set_stream_sample_rates(self.h, _ptr(ids), r.size, _ptr(r)))
+
+    def stream_sample_rates(self, stream_ids=None, n=None):
+        """The rate each listed stream runs at (default: streams 0..n-1, n = max_streams) -> int32[n]."""
+        ids = None if stream_ids is None else np.ascontiguousarray(stream_ids, dtype=np.int32).reshape(-1)
+        n = ids.size if ids is not None else (self.max_streams if n is None else n)
+        out = np.empty(n, dtype=np.int32)
+        self._check(self.api.lib.lyra_b200_stream_sample_rates(self.h, _ptr(ids), n, _ptr(out)))
+        return out
 
     @property
     def hop(self):

@@ -128,7 +128,7 @@ RvqDecodeKernel(const uint8_t* __restrict__ blob, RvqParams P, const uint8_t* __
 //                       import and copy set the offset so that the key travels with the stream.
 enum StreamStateKind { kStatePlain = 0, kStateCodecRs0 = 1, kStateCodecRs1 = 2, kStateCng = 3 };
 constexpr uint32_t kStateMagic = 0x5453594Cu;        // "LYST"
-constexpr uint32_t kStateVersion = 1;
+constexpr uint32_t kStateVersion = 2;                // 2: the per-stream sample rate (StreamRateKernel) joined the payload
 constexpr int kStateHeaderWords = 16;
 // header words: magic, version, record bytes, roles, sample rate, 0, model fingerprint (lo, hi), codec converter 0 / 1 live,
 // comfort-noise key (lo, hi), 0 x 4
@@ -286,6 +286,51 @@ StreamStateCopyKernel(StreamStateTable T, StreamIdChunk ids) {
 }
 
 // ------------------------------------------------------------------------------------------------
+// Per-stream sample rates of the fused codec calls (lyra_b200_set_stream_sample_rates).  Every stream has one state word: 0 =
+// the context's rate (lyra_b200_set_sample_rate), otherwise the stream's own rate (8000 / 16000 / 32000 / 48000, at most the
+// context's).  The converters (ResampleKernel) and the encoder-side DTX estimator (LogMelKernel, NoiseEstimatorKernel) read it.
+// Index of a rate in a per-rate table (ByRate): 0 = 16 kHz, 1 = 8 kHz, 2 = 32 kHz, 3 = 48 kHz (= the resampler's pair + 1).
+__host__ __device__ constexpr int RateIndex(int rate_hz) { return rate_hz == 8000 ? 1 : rate_hz == 32000 ? 2 : rate_hz == 48000 ? 3 : 0; }
+__device__ __forceinline__ int StreamRate(const int* __restrict__ rate_word, int stream, int ctx_rate) {
+  if (!rate_word) return ctx_rate;
+  const int w = rate_word[stream];
+  return w ? w : ctx_rate;
+}
+// One parameter set per rate, by RateIndex.  A caller with a single set passes it at every index (Uniform).
+template <typename T>
+struct ByRate { T p[4]; };
+template <typename T>
+ByRate<T> Uniform(const T& v) { return ByRate<T>{{v, v, v, v}}; }
+// the set of index k, selected field by field from the by-value kernel parameter (no dynamic indexing, so no local copy)
+template <typename T>
+__device__ __forceinline__ T PickByRate(const ByRate<T>& s, int k) {
+  T v = s.p[0];
+  if (k == 1) v = s.p[1];
+  if (k == 2) v = s.p[2];
+  if (k == 3) v = s.p[3];
+  return v;
+}
+
+// stream c.ids[k] <- rate c.rates[k] (validated by the host).  The word stores 0 for the context's rate.  A stream whose
+// effective rate changes gets {position, tag} = 0 in both codec converters (conv0 / conv1: nullptr when the context lacks that
+// role): tag 0 never matches, so each restarts fully primed on its next call, as a context-level change does.  The networks,
+// estimators and packet-loss state carry on.
+struct StreamRateChunk { int n; int ids[kStateChunk]; int rates[kStateChunk]; };
+constexpr int kStreamRateThreads = 256;
+
+__global__ void __launch_bounds__(kStreamRateThreads)
+StreamRateKernel(StreamRateChunk c, int ctx_rate, int* __restrict__ rate_word, int* __restrict__ conv0, int* __restrict__ conv1) {
+  const int k = (int)(blockIdx.x * blockDim.x + threadIdx.x);
+  if (k >= c.n) return;
+  const int s = c.ids[k], r = c.rates[k];
+  const int old = StreamRate(rate_word, s, ctx_rate);
+  rate_word[s] = r == ctx_rate ? 0 : r;
+  if (r == old) return;
+  if (conv0) { conv0[2 * (size_t)s] = 0; conv0[2 * (size_t)s + 1] = 0; }
+  if (conv1) { conv1[2 * (size_t)s] = 0; conv1[2 * (size_t)s + 1] = 0; }
+}
+
+// ------------------------------------------------------------------------------------------------
 // Log-mel spectrogram (LogMelSpectrogramExtractorImpl::Extract, lyra/log_mel_spectrogram_extractor_impl.cc:96-126).
 // One block of 128 threads per stream: periodic-Hann window over [previous hop, current hop], zero-padded 1024-point
 // radix-2 decimation-in-time FFT in double — the same butterflies, operand order and host-computed twiddles as the
@@ -338,10 +383,12 @@ __device__ __forceinline__ void FftStages3(double* re, double* im, int base, int
   for (int j = 0; j < 8; ++j) { re[FftIdx(base + j * STRIDE)] = xr[j]; im[FftIdx(base + j * STRIDE)] = xi[j]; }
 }
 
+// S: the extractor's tables by rate; each stream uses those of StreamRate(rate_word, stream, rate) (the encoder-side DTX
+// estimator follows the stream's rate); the sets differ only in their tables, not in hop, window or FFT size.
 __global__ void __launch_bounds__(kLogMelThreads)
-LogMelKernel(const uint8_t* __restrict__ blob, LogMelParams P, const int* __restrict__ stream_ids, int n,
-             const int16_t* __restrict__ pcm, int16_t* __restrict__ prev, float* __restrict__ out,
-             const uint8_t* __restrict__ mask, int slot_base) {
+LogMelKernel(const uint8_t* __restrict__ blob, ByRate<LogMelParams> S, const int* __restrict__ rate_word, int rate,
+             const int* __restrict__ stream_ids, int n, const int16_t* __restrict__ pcm, int16_t* __restrict__ prev,
+             float* __restrict__ out, const uint8_t* __restrict__ mask, int slot_base) {
   unsigned char* smem = LYRA_DYN_SMEM();
   double* re = reinterpret_cast<double*>(smem);
   double* im = re + kLogMelFftPadded;
@@ -351,6 +398,7 @@ LogMelKernel(const uint8_t* __restrict__ blob, LogMelParams P, const int* __rest
   if (slot >= n) return;
   if (mask && !mask[slot]) return;     // this stream's extractor is not fed this hop (its carried samples stay)
   const int stream = stream_ids ? stream_ids[slot] : slot;
+  const LogMelParams P = PickByRate(S, RateIndex(StreamRate(rate_word, stream, rate)));
   const int tid = (int)threadIdx.x;
   constexpr int NT = kLogMelThreads;
   const int carry = P.window_len - P.hop;
@@ -436,18 +484,20 @@ struct NoiseParams { int nf, hops_per_update; float max_smoothing, bound_decay; 
 constexpr int kNoiseThreads = 192;
 __host__ __device__ constexpr int NoiseStateUnits(int nf) { return 5 * nf + 4; }
 
+// S: the constants by rate, selected per stream as in LogMelKernel (every set has nf = 160 bins)
 __global__ void __launch_bounds__(kNoiseThreads)
-NoiseEstimatorKernel(NoiseParams P, const int* __restrict__ stream_ids, int n, const float* __restrict__ mel,
-                     const uint8_t* __restrict__ mask, float* __restrict__ state, uint8_t* __restrict__ is_noise_out,
-                     float* __restrict__ estimate_out, int slot_base) {
+NoiseEstimatorKernel(ByRate<NoiseParams> S, const int* __restrict__ rate_word, int rate, const int* __restrict__ stream_ids, int n,
+                     const float* __restrict__ mel, const uint8_t* __restrict__ mask, float* __restrict__ state,
+                     uint8_t* __restrict__ is_noise_out, float* __restrict__ estimate_out, int slot_base) {
+  const int slot = slot_base + (int)blockIdx.x;
+  if (slot >= n) return;
+  const int stream = stream_ids ? stream_ids[slot] : slot;
+  const NoiseParams P = PickByRate(S, RateIndex(StreamRate(rate_word, stream, rate)));
   unsigned char* smem = LYRA_DYN_SMEM();
   float* cur = reinterpret_cast<float*>(smem);       // [nf]
   float* sm = cur + P.nf;                             // [nf] smoothed power before this update
   float* red = sm + P.nf;                             // [0] smoothing correction
   int* flag = reinterpret_cast<int*>(red + 1);
-  const int slot = slot_base + (int)blockIdx.x;
-  if (slot >= n) return;
-  const int stream = stream_ids ? stream_ids[slot] : slot;
   const int i = (int)threadIdx.x, nf = P.nf;
   float* st = state + (size_t)stream * NoiseStateUnits(nf);
   float* est = st;

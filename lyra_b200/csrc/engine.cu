@@ -58,7 +58,7 @@ struct lyra_b200_ctx {
   // (nullptr: zero), hop counter `n18` (nullptr: none; initially 0).  `reset` = false: lyra_b200_reset leaves the entry alone
   // (lyra_b200_resample's delay lines).  `kind` (StreamStateKind) marks the words a record does not carry verbatim; `check`
   // is what import validates in a record's payload besides the hop counter.
-  enum Check { kCheckNone, kCheckPlc, kCheckResamplerPos };
+  enum Check { kCheckNone, kCheckPlc, kCheckResamplerPos, kCheckStreamRate };
   struct StateEntry {
     StreamStateEntry e;              // e.offset is set by BuildStateTable
     bool reset;
@@ -111,8 +111,11 @@ struct lyra_b200_ctx {
   int codec_rs_tag = 1;                          // ResampleKernel tag of the current setting (bumped by every change)
   int16_t* d_codec_rs_delay[2] = {nullptr, nullptr};
   int* d_codec_rs_pos[2] = {nullptr, nullptr};
-  NoiseParams enc_noise_params{};                // the encoder-side estimators' constants and extractor at sample_rate
-  const LogMelParams* enc_logmel = nullptr;
+  // lyra_b200_set_stream_sample_rates: one word per stream, 0 = sample_rate, otherwise the stream's own rate (StreamRateKernel)
+  int* d_stream_rate = nullptr;
+  bool rate_override = false;                    // some stream may run at another rate than sample_rate
+  ByRate<NoiseParams> enc_noise_params{};        // the encoder-side estimators' constants and extractor tables, by stream rate
+  ByRate<LogMelParams> enc_logmel{};
   // device staging for the host-buffer API
   int16_t* d_pcm = nullptr;
   uint8_t* d_packets = nullptr;
@@ -150,11 +153,14 @@ struct lyra_b200_ctx {
   uint64_t launches = 0;
   // lyra_b200_set_graphs: the dense host-buffer encode / decode calls replay a captured CUDA graph (copies in, kernels of every
   // sub-batch, copies out) instead of re-issuing ~20 stream operations per call; one graph per (call shape, host buffers)
+  // (rates: rate_override, which adds the converters' launches at 16 kHz)
   struct GraphKey {
     int kind, n, num_bits, mode, nsplit;
     const void *a, *b, *c;
+    bool rates;
     bool operator==(const GraphKey& o) const {
-      return kind == o.kind && n == o.n && num_bits == o.num_bits && mode == o.mode && nsplit == o.nsplit && a == o.a && b == o.b && c == o.c;
+      return kind == o.kind && n == o.n && num_bits == o.num_bits && mode == o.mode && nsplit == o.nsplit && a == o.a && b == o.b && c == o.c &&
+             rates == o.rates;
     }
   };
   struct GraphEntry { GraphKey key; void* exec; uint64_t launches; };
@@ -176,6 +182,10 @@ int PacketBytes(int num_bits) { return (num_bits + 7) / 8; }
 
 // index of an external rate in the resampler's filter banks (ResamplerParams pairs 0-2 to 16 kHz, 3-5 from it); -1: unsupported
 int RatePair(int rate_hz) { return rate_hz == 8000 ? 0 : rate_hz == 32000 ? 1 : rate_hz == 48000 ? 2 : -1; }
+bool RateOk(int rate_hz) { return rate_hz == 16000 || RatePair(rate_hz) >= 0; }
+
+// The fused codec calls convert when the context is not at 16 kHz or some stream may have a rate of its own
+bool Converts(const lyra_b200_ctx* ctx) { return ctx->sample_rate != 16000 || ctx->rate_override; }
 
 // NoiseEstimator::Create (lyra/noise_estimator.cc:99-120) for (rate_hz, hop 320, 160 features)
 NoiseParams MakeNoiseParams(int rate_hz) {
@@ -433,26 +443,34 @@ int JoinAfter(lyra_b200_ctx* ctx, int nparts, int rc) {
 
 // log-mel spectra of slots [slot0, slot0 + count) into ctx->d_melout on stream `st`, advancing the extractor state `carried`;
 // all arrays are indexed by slot, n = total slots of the call
-void LaunchLogMel(lyra_b200_ctx* ctx, cudaStream_t st, const LogMelParams& P, const int* d_ids, int slot0, int count, int n,
-                  const int16_t* d_pcm, int16_t* carried, const uint8_t* d_mask) {
+// S: the extractor's tables by rate, used per stream at StreamRate(rate_word, stream, rate) (one set: Uniform; the sets share
+// their sizes)
+void LaunchLogMel(lyra_b200_ctx* ctx, cudaStream_t st, const ByRate<LogMelParams>& S, const int* rate_word, int rate, const int* d_ids,
+                  int slot0, int count, int n, const int16_t* d_pcm, int16_t* carried, const uint8_t* d_mask) {
+  const LogMelParams& P = S.p[0];
   const size_t smem = sizeof(double) * (size_t)(2 * kLogMelFftPadded + P.fft / 2 + 1 + P.window_len + P.window_len / 8 + 1);
   ProfScope ps(ctx, 6, st);
   LYRA_LAUNCH(LogMelKernel, dim3((unsigned)count), dim3(kLogMelThreads), smem, st,
-              ctx->d_blob, P, d_ids, n, d_pcm, carried, ctx->d_melout, d_mask, slot0);
+              ctx->d_blob, S, rate_word, rate, d_ids, n, d_pcm, carried, ctx->d_melout, d_mask, slot0);
   ctx->launches += 1;
 }
 
 // log-mel of this hop (the estimator's own extractor, bank 2) + the estimator recurrences for slots
-// [slot0, slot0 + count) on stream `st`; all arrays are indexed by slot, n = total slots of the call
+// [slot0, slot0 + count) on stream `st`; all arrays are indexed by slot, n = total slots of the call.  The encoder side's
+// estimators are built for each stream's rate (NoiseEstimator::Create(rate, 320, 640, 160), lyra/lyra_encoder.cc:80-89); the
+// decoder side's stay at 16 kHz.
 int LaunchNoiseUpdate(lyra_b200_ctx* ctx, cudaStream_t st, const int* d_ids, int slot0, int count, int n, const int16_t* d_pcm,
                       const uint8_t* d_mask, uint8_t* d_is_noise, float* d_estimate, bool encoder_side = false) {
   float* noise_state = encoder_side ? ctx->d_noise_enc : ctx->d_noise;
   int16_t* carried = encoder_side ? ctx->d_logmel_prev_enc : ctx->d_logmel_prev[2];
-  LaunchLogMel(ctx, st, encoder_side ? *ctx->enc_logmel : ctx->spec.logmel160, d_ids, slot0, count, n, d_pcm, carried, d_mask);
+  const int* rate_word = encoder_side ? ctx->d_stream_rate : nullptr;
+  const int rate = encoder_side ? ctx->sample_rate : 16000;
+  LaunchLogMel(ctx, st, encoder_side ? ctx->enc_logmel : Uniform(ctx->spec.logmel160), rate_word, rate, d_ids, slot0, count, n, d_pcm,
+               carried, d_mask);
   { ProfScope ps(ctx, 7, st);
   LYRA_LAUNCH(NoiseEstimatorKernel, dim3((unsigned)count), dim3(kNoiseThreads), sizeof(float) * (size_t)(2 * 160 + 2), st,
-              encoder_side ? ctx->enc_noise_params : ctx->noise_params, d_ids, n, ctx->d_melout, d_mask, noise_state, d_is_noise,
-              d_estimate, slot0); }
+              encoder_side ? ctx->enc_noise_params : Uniform(ctx->noise_params), rate_word, rate, d_ids, n, ctx->d_melout, d_mask,
+              noise_state, d_is_noise, d_estimate, slot0); }
   ctx->launches += 1;
   CU(cudaGetLastError());
   return LYRA_B200_OK;
@@ -471,14 +489,15 @@ void LaunchComfortNoise(lyra_b200_ctx* ctx, cudaStream_t st, const int* d_ids, i
 
 // The codec path's sample-rate converter for the slots of part `p` (all arrays indexed by slot, n = total slots of the call):
 // dir 0 converts the external-rate rows `in` [n][rate / 50] to 16 kHz rows `out` [n][320] (the encoder's input side), dir 1 the
-// 16 kHz rows to external-rate rows (the decoder's output side).  Whole hops from phase 0 stay at phase 0 (the ratios are
-// integers), so every row is exactly one hop.
+// 16 kHz rows to external-rate rows (the decoder's output side).  Each stream converts at its own rate (d_stream_rate; rows of a
+// stream below the context's rate use their first rate / 50 samples, decoder rows get zeros after them).  Whole hops from phase
+// 0 stay at phase 0 (the ratios are integers), so every row is exactly one hop.
 int LaunchCodecResample(lyra_b200_ctx* ctx, const Part& p, int dir, const int* d_ids, int n, const int16_t* in, int16_t* out) {
-  const int ext = ctx->sample_rate / 50, pair = RatePair(ctx->sample_rate) + (dir ? 3 : 0);
-  const int n_in = dir ? LYRA_B200_HOP : ext, n_out = dir ? ext : LYRA_B200_HOP;
-  LYRA_LAUNCH(ResampleKernel, dim3((unsigned)p.nslots), dim3(128), sizeof(float) * (size_t)(kResamplerTaps - 1 + n_in), p.st,
-              ctx->d_blob, ctx->spec.resampler, pair, ctx->codec_rs_tag, d_ids, n, in, n_in, out, n_out, nullptr,
-              ctx->d_codec_rs_delay[dir], ctx->d_codec_rs_pos[dir], p.slot0);
+  const int ext = ctx->sample_rate / 50;
+  const int in_stride = dir ? LYRA_B200_HOP : ext, out_stride = dir ? ext : LYRA_B200_HOP;
+  LYRA_LAUNCH(ResampleKernel, dim3((unsigned)p.nslots), dim3(128), sizeof(float) * (size_t)(kResamplerTaps - 1 + in_stride), p.st,
+              ctx->d_blob, ctx->spec.resampler, dir ? 3 : 0, ctx->codec_rs_tag, d_ids, n, in, in_stride, in_stride, out, out_stride,
+              nullptr, ctx->d_codec_rs_delay[dir], ctx->d_codec_rs_pos[dir], p.slot0, ctx->d_stream_rate, ctx->sample_rate);
   ctx->launches += 1;
   CU(cudaGetLastError());
   return LYRA_B200_OK;
@@ -498,7 +517,7 @@ int RunEncode(lyra_b200_ctx* ctx, int n, const int16_t* d_pcm, int num_bits, uin
   Part parts[lyra_b200_ctx::kMaxSplit];
   const int np = SplitParts(ctx, n, parts);
   const size_t pb = (size_t)PacketBytes(num_bits), hop = (size_t)ctx->sample_rate / 50;
-  const bool rs = ctx->sample_rate != 16000;
+  const bool rs = Converts(ctx);
   int16_t* stage = rs ? ctx->d_rs_in : ctx->d_pcm;      // where a host-buffer call's rows land
   const int16_t* in = h_pcm ? stage : d_pcm;
   const int16_t* pcm16 = rs ? ctx->d_pcm : in;
@@ -537,7 +556,7 @@ int RunDecode(lyra_b200_ctx* ctx, int n, const uint8_t* d_packets, const uint8_t
   Part parts[lyra_b200_ctx::kMaxSplit];
   const int np = SplitParts(ctx, n, parts);
   const size_t pb = (size_t)PacketBytes(num_bits), hop = (size_t)ctx->sample_rate / 50;
-  const bool rs = ctx->sample_rate != 16000;
+  const bool rs = Converts(ctx);
   int16_t* out = h_pcm && rs ? ctx->d_rs_out : d_pcm;
   int16_t* pcm16 = rs ? ctx->d_pcm : out;
   int rc = Fork(ctx, np);
@@ -570,7 +589,7 @@ int RunDecode(lyra_b200_ctx* ctx, int n, const uint8_t* d_packets, const uint8_t
 int RunDecodePlc(lyra_b200_ctx* ctx, int n, const uint8_t* d_packets, const uint8_t* d_received, int num_bits, int16_t* d_pcm,
                  const int* d_ids, uint8_t* d_is_cn, const uint8_t* h_packets, const uint8_t* h_received, int16_t* h_pcm, uint8_t* h_is_cn) {
   const size_t pb = (size_t)PacketBytes(num_bits), hop = (size_t)ctx->sample_rate / 50;
-  const bool rs = ctx->sample_rate != 16000;
+  const bool rs = Converts(ctx);
   int16_t* out = h_pcm && rs ? ctx->d_rs_out : d_pcm;
   int16_t* pcm16 = rs ? ctx->d_pcm : out;
   if (h_received) CU(cudaMemcpyAsync(ctx->d_received, h_received, (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
@@ -781,6 +800,9 @@ bool PlcStateOk(int cp, int fp, int dir) {
          (dir == 1 || dir == -1);
 }
 
+// a rate lyra_b200_set_stream_sample_rates accepts: supported, and its hop fits the context's rows
+bool StreamRateOk(const lyra_b200_ctx* ctx, int rate_hz) { return RateOk(rate_hz) && rate_hz <= ctx->sample_rate; }
+
 uint32_t RecordWord(const uint8_t* rec, int i) {
   uint32_t w;
   std::memcpy(&w, rec + 4 * (size_t)i, 4);
@@ -811,6 +833,8 @@ const char* RecordProblem(const lyra_b200_ctx* ctx, const uint8_t* rec) {
     if (check == lyra_b200_ctx::kCheckPlc &&
         !PlcStateOk((int32_t)RecordWord(rec, w0), (int32_t)RecordWord(rec, w0 + 1), (int32_t)RecordWord(rec, w0 + 2)))
       return "decoder control state out of range";
+    if (check == lyra_b200_ctx::kCheckStreamRate && RecordWord(rec, w0) != 0 && !StreamRateOk(ctx, (int32_t)RecordWord(rec, w0)))
+      return "stream sample rate unsupported or above the context's";
   }
   return nullptr;
 }
@@ -853,6 +877,24 @@ int CopyStreamState(lyra_b200_ctx* ctx, const StreamStateTable& T, const int32_t
       ids.dst[k] = dst ? dst[k0 + k] : k0 + k;
     }
     LYRA_LAUNCH(StreamStateCopyKernel, StateGrid(T, ids.n, 0), dim3(kStateThreads), (size_t)0, ctx->stream, T, ids);
+    ctx->launches += 1;
+  }
+  CU(cudaGetLastError());
+  return LYRA_B200_OK;
+}
+
+// StreamRateKernel on ctx->stream, one launch per kStateChunk streams: stream ids[k] (nullptr: k) <- rates[k] (nullptr: the
+// context's rate).  Ids and rates travel as kernel parameters.
+int LaunchStreamRates(lyra_b200_ctx* ctx, const int32_t* ids, int n, const int32_t* rates) {
+  StreamRateChunk c;
+  for (int k0 = 0; k0 < n; k0 += kStateChunk) {
+    c.n = n - k0 < kStateChunk ? n - k0 : kStateChunk;
+    for (int k = 0; k < c.n; ++k) {
+      c.ids[k] = ids ? ids[k0 + k] : k0 + k;
+      c.rates[k] = rates ? rates[k0 + k] : ctx->sample_rate;
+    }
+    LYRA_LAUNCH(StreamRateKernel, dim3((unsigned)((c.n + kStreamRateThreads - 1) / kStreamRateThreads)), dim3(kStreamRateThreads),
+                (size_t)0, ctx->stream, c, ctx->sample_rate, ctx->d_stream_rate, ctx->d_codec_rs_pos[0], ctx->d_codec_rs_pos[1]);
     ctx->launches += 1;
   }
   CU(cudaGetLastError());
@@ -936,8 +978,10 @@ int lyra_b200_create_ex(const char* model_dir, int device, int max_streams, int 
   if (roles & LYRA_B200_ROLE_DECODER) ok = ok && DevAlloc(ctx, &ctx->d_mid_dec, P * 128 * 4);
   for (int b = 0; b < 3; ++b) ok = ok && DevStreamState(ctx, &ctx->d_logmel_prev[b], LYRA_B200_HOP);
   ctx->noise_params = MakeNoiseParams(16000);
-  ctx->enc_noise_params = ctx->noise_params;
-  ctx->enc_logmel = &ctx->spec.logmel160;
+  for (int r : {16000, 8000, 32000, 48000}) {
+    ctx->enc_noise_params.p[RateIndex(r)] = MakeNoiseParams(r);
+    ctx->enc_logmel.p[RateIndex(r)] = r == 16000 ? ctx->spec.logmel160 : ctx->spec.logmel160_ext[RatePair(r)];
+  }
   // noise estimators: all-zero is the freshly constructed object
   ok = ok && DevStreamState(ctx, &ctx->d_noise, NoiseStateUnits(160));
   ok = ok && DevAlloc(ctx, &ctx->d_noise_est, P * 160);
@@ -970,6 +1014,8 @@ int lyra_b200_create_ex(const char* model_dir, int device, int max_streams, int 
     ok = ok && DevStreamState(ctx, &ctx->d_codec_rs_pos[d], 2, nullptr, d == 0 ? kStateCodecRs0 : kStateCodecRs1,
                               lyra_b200_ctx::kCheckResamplerPos);
   }
+  // the stream's own sample rate (lyra_b200_set_stream_sample_rates): 0, the context's, at creation and after reset
+  ok = ok && DevStreamState(ctx, &ctx->d_stream_rate, 1, nullptr, kStatePlain, lyra_b200_ctx::kCheckStreamRate);
   ok = ok && DevAlloc(ctx, &ctx->d_rs_in, P * 960);
   ok = ok && DevAlloc(ctx, &ctx->d_rs_out, P * 968);
   ok = ok && DevAlloc(ctx, &ctx->d_rs_counts, P);
@@ -1129,18 +1175,62 @@ int lyra_b200_decoder_mode(const lyra_b200_ctx* ctx) { return ctx ? ctx->decoder
 
 int lyra_b200_set_sample_rate(lyra_b200_ctx* ctx, int sample_rate_hz) {
   if (!ctx) return LYRA_B200_EINVAL;
-  const int pair = RatePair(sample_rate_hz);
-  if (sample_rate_hz != 16000 && pair < 0) { ctx->err = "the codec calls run at 8000, 16000, 32000 or 48000 Hz"; return LYRA_B200_EINVAL; }
+  if (!RateOk(sample_rate_hz)) { ctx->err = "the codec calls run at 8000, 16000, 32000 or 48000 Hz"; return LYRA_B200_EINVAL; }
   ENTER(0);
-  if (sample_rate_hz == ctx->sample_rate) return LYRA_B200_OK;
+  if (sample_rate_hz == ctx->sample_rate && !ctx->rate_override) return LYRA_B200_OK;
   CU(SyncStream(ctx));
+  if (sample_rate_hz == ctx->sample_rate) {
+    // the same rate: the streams with a rate of their own come back to it (their converters restart), the others are untouched
+    int rc = LaunchStreamRates(ctx, nullptr, ctx->max_streams, nullptr);
+    if (rc) return rc;
+    CU(SyncStream(ctx));
+    ctx->rate_override = false;
+    return LYRA_B200_OK;
+  }
 #ifndef LYRA_EMU
   DropGraphs(ctx);                   // captured graphs carry the converters' rate, tag and row sizes
 #endif
+  if (ctx->rate_override) {
+    CU(cudaMemsetAsync(ctx->d_stream_rate, 0, sizeof(int) * (size_t)ctx->padded, ctx->stream));   // every stream at the new rate
+    CU(SyncStream(ctx));
+    ctx->rate_override = false;
+  }
   ctx->sample_rate = sample_rate_hz;
   ctx->codec_rs_tag = ctx->codec_rs_tag % 1000000000 + 1;    // every stream's converters restart primed on their next call
-  ctx->enc_logmel = pair < 0 ? &ctx->spec.logmel160 : &ctx->spec.logmel160_ext[pair];
-  ctx->enc_noise_params = MakeNoiseParams(sample_rate_hz);
+  return LYRA_B200_OK;
+}
+
+int lyra_b200_set_stream_sample_rates(lyra_b200_ctx* ctx, const int32_t* stream_ids, int n, const int32_t* rates_hz) {
+  if (!ctx || !rates_hz) return LYRA_B200_EINVAL;
+  ENTER(0);
+  int rc = CheckIds(ctx, stream_ids, n, false);
+  if (rc) return rc;
+  bool differs = false;
+  for (int k = 0; k < n; ++k) {
+    if (!StreamRateOk(ctx, rates_hz[k])) {
+      ctx->err = "a stream runs at 8000, 16000, 32000 or 48000 Hz, at most the context's rate (lyra_b200_set_sample_rate)";
+      return LYRA_B200_EINVAL;
+    }
+    differs |= rates_hz[k] != ctx->sample_rate;
+  }
+  if (!differs && !ctx->rate_override) return LYRA_B200_OK;     // every stream is at the context's rate already
+  if ((rc = LaunchStreamRates(ctx, stream_ids, n, rates_hz))) return rc;
+  ctx->rate_override = true;
+  return LYRA_B200_OK;
+}
+
+int lyra_b200_stream_sample_rates(lyra_b200_ctx* ctx, const int32_t* stream_ids, int n, int32_t* rates_hz) {
+  if (!ctx || !rates_hz) return LYRA_B200_EINVAL;
+  ENTER(0);
+  const int rc = CheckIds(ctx, stream_ids, n, true);
+  if (rc) return rc;
+  CU(SyncStream(ctx));
+  std::vector<int> words((size_t)ctx->max_streams);
+  CU(cudaMemcpy(words.data(), ctx->d_stream_rate, sizeof(int) * words.size(), cudaMemcpyDeviceToHost));
+  for (int k = 0; k < n; ++k) {
+    const int w = words[(size_t)(stream_ids ? stream_ids[k] : k)];
+    rates_hz[k] = w ? w : ctx->sample_rate;
+  }
   return LYRA_B200_OK;
 }
 
@@ -1190,8 +1280,8 @@ int lyra_b200_encode(lyra_b200_ctx* ctx, const int32_t* ids, int n, const int16_
   if (!BitsOk(ctx, num_bits)) return LYRA_B200_EINVAL;
   const int* d_ids = nullptr;      // the codec resampler's state is per stream: a sparse call at another rate needs the ids
   int rc = PrepareMap(ctx, ids, n);
-  if (rc || (ctx->sample_rate != 16000 && (rc = UploadIds(ctx, ids, n, &d_ids)))) return rc;
-  const lyra_b200_ctx::GraphKey key{0, n, num_bits, 0, ctx->nsplit, pcm, packets, nullptr};
+  if (rc || (Converts(ctx) && (rc = UploadIds(ctx, ids, n, &d_ids)))) return rc;
+  const lyra_b200_ctx::GraphKey key{0, n, num_bits, 0, ctx->nsplit, pcm, packets, nullptr, ctx->rate_override};
   if ((rc = RunMaybeGraphed(ctx, key, ids == nullptr && ctx->map_dense_n == n,
                             [&]() { return RunEncode(ctx, n, ctx->d_pcm, num_bits, ctx->d_packets, pcm, packets, false, d_ids); })))
     return rc;
@@ -1206,8 +1296,8 @@ int lyra_b200_decode(lyra_b200_ctx* ctx, const int32_t* ids, int n, const uint8_
   if (!BitsOk(ctx, num_bits)) return LYRA_B200_EINVAL;
   const int* d_ids = nullptr;
   int rc = PrepareMap(ctx, ids, n);
-  if (rc || (ctx->sample_rate != 16000 && (rc = UploadIds(ctx, ids, n, &d_ids)))) return rc;
-  const lyra_b200_ctx::GraphKey key{1, n, num_bits, ctx->decoder_mode, ctx->nsplit, packets, received, pcm};
+  if (rc || (Converts(ctx) && (rc = UploadIds(ctx, ids, n, &d_ids)))) return rc;
+  const lyra_b200_ctx::GraphKey key{1, n, num_bits, ctx->decoder_mode, ctx->nsplit, packets, received, pcm, ctx->rate_override};
   if ((rc = RunMaybeGraphed(ctx, key, ids == nullptr && ctx->map_dense_n == n, [&]() {
          return RunDecode(ctx, n, ctx->d_packets, received ? ctx->d_received : nullptr, num_bits, ctx->d_pcm, packets, received, pcm,
                           false, d_ids);
@@ -1282,7 +1372,7 @@ int lyra_b200_logmel(lyra_b200_ctx* ctx, int bank, const int32_t* ids, int n, co
   if (rc || (rc = UploadIds(ctx, ids, n, &d_ids))) return rc;
   const LogMelParams& P = num_mel_bins == 160 ? ctx->spec.logmel160 : ctx->spec.logmel64;
   CU(cudaMemcpyAsync(ctx->d_pcm, pcm, sizeof(int16_t) * 320 * (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
-  LaunchLogMel(ctx, ctx->stream, P, d_ids, 0, n, n, ctx->d_pcm, ctx->d_logmel_prev[bank], nullptr);
+  LaunchLogMel(ctx, ctx->stream, Uniform(P), nullptr, 16000, d_ids, 0, n, n, ctx->d_pcm, ctx->d_logmel_prev[bank], nullptr);
   CU(cudaGetLastError());
   CU(cudaMemcpyAsync(out, ctx->d_melout, sizeof(float) * (size_t)num_mel_bins * (size_t)n, cudaMemcpyDeviceToHost, ctx->stream));
   CU(SyncStream(ctx));
@@ -1461,8 +1551,8 @@ int lyra_b200_resample(lyra_b200_ctx* ctx, int to_internal, const int32_t* ids, 
   CU(cudaMemcpyAsync(ctx->d_rs_in, in, sizeof(int16_t) * (size_t)in_samples * (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
   const int dir = to_internal ? 0 : 1;
   LYRA_LAUNCH(ResampleKernel, dim3((unsigned)n), dim3(128), sizeof(float) * (size_t)(kResamplerTaps - 1 + in_samples), ctx->stream,
-              ctx->d_blob, ctx->spec.resampler, pr, external_rate_hz, d_ids, n, ctx->d_rs_in, in_samples, ctx->d_rs_out, out_stride,
-              ctx->d_rs_counts, ctx->d_rs_delay[dir], ctx->d_rs_pos[dir], 0);
+              ctx->d_blob, ctx->spec.resampler, pr, external_rate_hz, d_ids, n, ctx->d_rs_in, in_samples, in_samples, ctx->d_rs_out,
+              out_stride, ctx->d_rs_counts, ctx->d_rs_delay[dir], ctx->d_rs_pos[dir], 0, nullptr, external_rate_hz);
   ctx->launches += 1;
   CU(cudaGetLastError());
   CU(cudaMemcpyAsync(out, ctx->d_rs_out, sizeof(int16_t) * (size_t)out_stride * (size_t)n, cudaMemcpyDeviceToHost, ctx->stream));
@@ -1503,12 +1593,18 @@ int lyra_b200_import_streams(lyra_b200_ctx* ctx, const int32_t* stream_ids, int 
   if (rc) return rc;
   const size_t rb = RecordBytes(ctx);
   const uint8_t* recs = static_cast<const uint8_t*>(records);
-  for (int k = 0; k < n; ++k)                      // every record first: a bad one changes nothing
+  bool own_rate = false;
+  for (int k = 0; k < n; ++k) {                    // every record first: a bad one changes nothing
     if (const char* why = RecordProblem(ctx, recs + rb * (size_t)k)) {
       ctx->err = "record " + std::to_string(k) + ": " + why;
       return LYRA_B200_EINVAL;
     }
+    for (size_t i = 0; i < ctx->state_list.size(); ++i)
+      if (ctx->state_list[i].check == lyra_b200_ctx::kCheckStreamRate)
+        own_rate |= RecordWord(recs + rb * (size_t)k, kStateHeaderWords + ctx->state_list[i].e.offset) != 0;
+  }
   if ((rc = EnsureRecordStaging(ctx))) return rc;
+  if (own_rate) ctx->rate_override = true;
   StreamIdChunk ids;
   for (int k0 = 0; k0 < n; k0 += ctx->records_chunk) {
     ids.n = n - k0 < ctx->records_chunk ? n - k0 : ctx->records_chunk;

@@ -214,11 +214,17 @@ NoiseReadKernel(const int* __restrict__ stream_ids, int n, const float* __restri
 // the external rate; the codec path: the generation of the context's rate setting).  A call with another tag starts from the
 // fully-primed state, like a fresh Resampler; 0 (what lyra_b200_reset writes) never matches.  counts[slot] (may be nullptr) =
 // outputs produced (they differ by at most one between streams when down-sampling from different phases).  I/O arrays are indexed
-// by slot: block b handles slot slot_base + b of a call of n slots; in rows are n_in samples and out rows `out_stride` samples apart.
+// by slot: block b handles slot slot_base + b of a call of n slots; in rows are `in_stride` and out rows `out_stride` samples apart.
+// rate_word == nullptr (lyra_b200_resample): every stream converts n_in samples with `pair`, at most out_stride outputs.
+// rate_word != nullptr (the fused codec calls, one whole hop per row): pair is 0 (to 16 kHz) or 3 (from 16 kHz) and each stream
+// runs at its own rate r = StreamRate(rate_word, stream, rate) (`rate` = the context's): pair + RateIndex(r) - 1, r / 50 samples on
+// the external side, 320 on the 16 kHz side; a 16 kHz stream is copied through and its converter state is left alone.  Output rows
+// longer than the stream's hop (a decoder row of a stream below the context's rate) get zeros after it.
 __global__ void __launch_bounds__(128)
 ResampleKernel(const uint8_t* __restrict__ blob, ResamplerParams P, int pair, int tag, const int* __restrict__ stream_ids, int n,
-               const int16_t* __restrict__ in, int n_in, int16_t* __restrict__ out, int out_stride, int* __restrict__ counts,
-               int16_t* __restrict__ delay_state, int* __restrict__ pos_state, int slot_base) {
+               const int16_t* __restrict__ in, int in_stride, int n_in, int16_t* __restrict__ out, int out_stride,
+               int* __restrict__ counts, int16_t* __restrict__ delay_state, int* __restrict__ pos_state, int slot_base,
+               const int* __restrict__ rate_word, int rate) {
   unsigned char* smem = LYRA_DYN_SMEM();
   float* x = reinterpret_cast<float*>(smem);              // [34 + n_in]: delay line followed by the new samples
   const int slot = slot_base + (int)blockIdx.x;
@@ -226,18 +232,34 @@ ResampleKernel(const uint8_t* __restrict__ blob, ResamplerParams P, int pair, in
   const int stream = stream_ids ? stream_ids[slot] : slot;
   constexpr int T = kResamplerTaps;
   const int tid = (int)threadIdx.x, NT = (int)blockDim.x;
+  const int16_t* row = in + (size_t)slot * in_stride;
+  int16_t* orow = out + (size_t)slot * out_stride;
+  int n_out = out_stride;
+  if (rate_word) {
+    constexpr int H = 320;                                // one 16 kHz hop
+    const int r = StreamRate(rate_word, stream, rate), k = RateIndex(r);
+    if (k == 0) {                                         // 16 kHz: no conversion
+      for (int j = tid; j < out_stride; j += NT) orow[j] = j < H ? row[j] : (int16_t)0;
+      return;
+    }
+    n_in = pair < 3 ? r / 50 : H;
+    n_out = pair < 3 ? H : r / 50;
+    pair += k - 1;
+  }
   int16_t* dl = delay_state + (size_t)stream * (T - 1);
   int* ps = pos_state + (size_t)stream * 2;              // {pos, tag}
   const bool fresh = ps[1] != tag;
   const int a0 = fresh ? 0 : ps[0];
   for (int i = tid; i < T - 1; i += NT) x[i] = fresh ? 0.0f : (float)dl[i];
-  for (int i = tid; i < n_in; i += NT) x[T - 1 + i] = (float)in[(size_t)slot * n_in + i];
+  for (int i = tid; i < n_in; i += NT) x[T - 1 + i] = (float)row[i];
   __syncthreads();
   const int num = P.num[pair], den = P.den[pair];
   const float* coeffs = BlobPtr<float>(blob, P.coeffs[pair]);
   const int total = n_in * den;
   const int count = a0 < total ? (total - a0 + num - 1) / num : 0;
-  for (int j = tid; j < count && j < out_stride; j += NT) {
+  if (rate_word)
+    for (int j = (count < n_out ? count : n_out) + tid; j < out_stride; j += NT) orow[j] = 0;
+  for (int j = tid; j < count && j < n_out; j += NT) {
     const int a = a0 + j * num, i = a / den, ph = a % den;
     const float* c = coeffs + ph * T;
     const float* xs = x + i;                              // delay-line sample 0 of the window that ends at input sample i
@@ -247,7 +269,7 @@ ResampleKernel(const uint8_t* __restrict__ blob, ResamplerParams P, int pair, in
     float v = acc;
     v = v > -32768.0f ? v : -32768.0f;
     v = v < 32767.0f ? v : 32767.0f;
-    out[(size_t)slot * out_stride + j] = (int16_t)v;
+    orow[j] = (int16_t)v;
   }
   __syncthreads();
   for (int i = tid; i < T - 1; i += NT) dl[i] = (int16_t)x[n_in + i];     // the last 34 samples of [delay | in]
