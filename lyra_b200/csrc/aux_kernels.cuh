@@ -357,8 +357,9 @@ __device__ __forceinline__ int FftIdx(int i) { return i + (i >> 3); }
 constexpr int kLogMelFftPadded = kLogMelFft + kLogMelFft / 8;
 
 // three consecutive stages (half-lengths STRIDE, 2 STRIDE, 4 STRIDE) on the 8 points base + j * STRIDE; r = base mod STRIDE.
-// tw: per-stage twiddle tables, the stage of half-length h starts at complex entry h - 1.
-template <int STRIDE>
+// tw: per-stage twiddle tables, the stage of half-length h starts at complex entry h - 1.  INV: the inverse transform's stages
+// (conjugated twiddles).
+template <int STRIDE, bool INV>
 __device__ __forceinline__ void FftButterflies3(double (&xr)[8], double (&xi)[8], int r, const double2* __restrict__ tw) {
 #pragma unroll
   for (int s = 0; s < 3; ++s) {
@@ -368,19 +369,51 @@ __device__ __forceinline__ void FftButterflies3(double (&xr)[8], double (&xi)[8]
       if (!(j & (1 << s))) {
         const int k = r + (j & ((1 << s) - 1)) * STRIDE;
         const double2 w = tw[half - 1 + k];
-        FftButterfly(xr[j], xi[j], xr[j + (1 << s)], xi[j + (1 << s)], w.x, w.y);
+        FftButterfly(xr[j], xi[j], xr[j + (1 << s)], xi[j + (1 << s)], w.x, INV ? -w.y : w.y);
       }
   }
 }
 
-template <int STRIDE>
+template <int STRIDE, bool INV>
 __device__ __forceinline__ void FftStages3(double* re, double* im, int base, int r, const double2* __restrict__ tw) {
   double xr[8], xi[8];
 #pragma unroll
   for (int j = 0; j < 8; ++j) { xr[j] = re[FftIdx(base + j * STRIDE)]; xi[j] = im[FftIdx(base + j * STRIDE)]; }
-  FftButterflies3<STRIDE>(xr, xi, r, tw);
+  FftButterflies3<STRIDE, INV>(xr, xi, r, tw);
 #pragma unroll
   for (int j = 0; j < 8; ++j) { re[FftIdx(base + j * STRIDE)] = xr[j]; im[FftIdx(base + j * STRIDE)] = xi[j]; }
+}
+
+// The whole 1024-point transform, run by one block of 128 threads: re / im (FftIdx layout) receive the spectrum (the signal if
+// INV, unscaled) of the points that gather(i, xr, xi) reads in natural order i.  Ends with a block barrier.
+template <bool INV, typename Gather>
+__device__ __forceinline__ void Fft1024(double* re, double* im, const double2* __restrict__ tw, Gather gather) {
+  constexpr int NT = 128;
+  const int tid = (int)threadIdx.x;
+  {                                                                            // stages 2, 4, 8 on points 8 tid .. 8 tid + 7
+    double xr[8], xi[8];
+    const int b7 = (int)(__brev((unsigned)tid) >> 25);                         // bit-reversed position 8t + j <-> natural index brev7(t) + 128 brev3(j)
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const int j3 = ((j & 1) << 2) | (j & 2) | ((j & 4) >> 2);
+      gather(b7 + 128 * j3, xr[j], xi[j]);
+    }
+    FftButterflies3<1, INV>(xr, xi, 0, tw);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) { re[FftIdx(8 * tid + j)] = xr[j]; im[FftIdx(8 * tid + j)] = xi[j]; }
+  }
+  __syncthreads();
+  FftStages3<8, INV>(re, im, 64 * (tid / 8) + tid % 8, tid % 8, tw);           // stages 16, 32, 64
+  __syncthreads();
+  FftStages3<64, INV>(re, im, 512 * (tid / 64) + tid % 64, tid % 64, tw);      // stages 128, 256, 512
+  __syncthreads();
+#pragma unroll
+  for (int m = 0; m < 4; ++m) {                                                // stage 1024
+    const int a = tid + NT * m, ia = FftIdx(a), ib = FftIdx(a + 512);
+    const double2 w = tw[511 + a];
+    FftButterfly(re[ia], im[ia], re[ib], im[ib], w.x, INV ? -w.y : w.y);
+  }
+  __syncthreads();
 }
 
 // S: the extractor's tables by rate; each stream uses those of StreamRate(rate_word, stream, rate) (the encoder-side DTX
@@ -422,32 +455,10 @@ LogMelKernel(const uint8_t* __restrict__ blob, ByRate<LogMelParams> S, const int
     __syncthreads();
     for (int i = tid; i < carry; i += NT) pv[i] = stage[i];
   }
-  {                                                                            // stages 2, 4, 8 on points 8 tid .. 8 tid + 7
-    double xr[8], xi[8];
-    const int b7 = (int)(__brev((unsigned)tid) >> 25);                         // bit-reversed position 8t + j <-> natural index brev7(t) + 128 brev3(j)
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const int j3 = ((j & 1) << 2) | (j & 2) | ((j & 4) >> 2);
-      const int i = b7 + 128 * j3;
-      xr[j] = i < P.window_len ? xw[FftIdx(i)] : 0.0;
-      xi[j] = 0.0;
-    }
-    FftButterflies3<1>(xr, xi, 0, tw);
-#pragma unroll
-    for (int j = 0; j < 8; ++j) { re[FftIdx(8 * tid + j)] = xr[j]; im[FftIdx(8 * tid + j)] = xi[j]; }
-  }
-  __syncthreads();
-  FftStages3<8>(re, im, 64 * (tid / 8) + tid % 8, tid % 8, tw);                // stages 16, 32, 64
-  __syncthreads();
-  FftStages3<64>(re, im, 512 * (tid / 64) + tid % 64, tid % 64, tw);           // stages 128, 256, 512
-  __syncthreads();
-#pragma unroll
-  for (int m = 0; m < 4; ++m) {                                                // stage 1024
-    const int a = tid + NT * m, ia = FftIdx(a), ib = FftIdx(a + 512);
-    const double2 w = tw[511 + a];
-    FftButterfly(re[ia], im[ia], re[ib], im[ib], w.x, w.y);
-  }
-  __syncthreads();
+  Fft1024<false>(re, im, tw, [&](int i, double& xr, double& xi) {
+    xr = i < P.window_len ? xw[FftIdx(i)] : 0.0;
+    xi = 0.0;
+  });
   const int bins = kLogMelFft / 2 + 1;
   for (int i = tid; i < bins; i += NT)
     mag[i] = __dsqrt_rn(__dadd_rn(__dmul_rn(re[FftIdx(i)], re[FftIdx(i)]), __dmul_rn(im[FftIdx(i)], im[FftIdx(i)])));

@@ -927,23 +927,6 @@ int LaunchStreamRates(lyra_b200_ctx* ctx, const int32_t* ids, int n, const int32
 
 }  // namespace
 
-#if defined(LYRA_PHASE_PROF) && !defined(LYRA_EMU)
-// development aid: returns clock64() stamps [4 kernels][1024 blocks][48 phases] of the most recent launches
-extern "C" int lyra_b200_debug_phases(lyra_b200_ctx* ctx, long long* out) {
-  static long long* d_buf = nullptr;
-  const size_t n = (size_t)4 * 1024 * 48;
-  if (!d_buf) {
-    cudaMalloc(reinterpret_cast<void**>(&d_buf), n * sizeof(long long));
-    cudaMemset(d_buf, 0, n * sizeof(long long));
-    cudaMemcpyToSymbol(lyra_b200::g_phase_prof, &d_buf, sizeof(d_buf));
-    return 1;
-  }
-  cudaStreamSynchronize(ctx->stream);
-  cudaMemcpy(out, d_buf, n * sizeof(long long), cudaMemcpyDeviceToHost);
-  return 0;
-}
-#endif
-
 extern "C" {
 
 int lyra_b200_create(const char* model_dir, int device, int max_streams, lyra_b200_ctx** out) {

@@ -22,14 +22,6 @@ namespace lyra_b200 {
 // DecoderKernelDW's warp-to-row mapping are all sized for it.
 constexpr int kTileStreams = 8;
 
-// Development aid (-DLYRA_PHASE_PROF): thread 0 of every block stamps clock64() at phase boundaries.
-#if defined(LYRA_PHASE_PROF) && !defined(LYRA_EMU)
-__device__ long long* g_phase_prof = nullptr;
-#define LYRA_PHASE(k, ph) do { if (threadIdx.x == 0 && g_phase_prof && blockIdx.x < 1024) g_phase_prof[((size_t)(k) * 1024 + blockIdx.x) * 48 + (ph)] = clock64(); ++(ph); } while (0)
-#else
-#define LYRA_PHASE(k, ph) do { (void)(ph); } while (0)
-#endif
-
 // ---- per-tile state layouts, in 4-byte units (each unit is S lanes wide) ----
 struct EncStateA {
   static constexpr int kFirst = 0;                               // [48]
@@ -105,6 +97,35 @@ __device__ __forceinline__ void PrefetchTileState(const void* p, int bytes) {
   if (threadIdx.x == 0) lyra_prefetch_l2(p, (unsigned)bytes);
 }
 
+// The prologue of every conv-net kernel, after its own weight-pipe or mbarrier setup: the tile's metadata into shared memory at
+// meta = slot[S], active[S], n18[S + 1], then its state block (`units` 4-byte units per lane of `state`) into the L2.
+// Returns false if the tile is idle.  It stays a composition of the two functions above: the same steps written inline give
+// different PTX register numbering, and ptxas then allocates differently (kernels B and D spilled other amounts).
+template <int S>
+__device__ __forceinline__ bool BeginTile(const TileIo& io, const int* n18g, int* meta, float* state, int units, int& tile) {
+  LoadTileMeta<S>(io, n18g, meta, meta + S, meta + 2 * S, tile);
+  if (meta[3 * S] == kTileIdle) return false;
+  PrefetchTileState(state + (size_t)tile * units * S, units * S * 4);
+  return true;
+}
+
+// The epilogue of every conv-net kernel: the frame counter of each active stream of the tile advances by one hop
+template <int S>
+__device__ __forceinline__ void AdvanceHopCounters(int* n18g, int tile, const int* active, const int* n18) {
+  const int tid = (int)threadIdx.x;
+  if (tid < S && active[tid]) n18g[tile * S + tid] = (n18[tid] + 1) % 18;
+}
+
+// The newest R rows of a [C][ld] shared-memory buffer, rows row0 .. row0 + R - 1, become the carried rows [C][R] of the
+// active streams: state unit `unit` onwards of the tile's state block st
+template <int S, int NT, int C, int R, typename T>
+__device__ __forceinline__ void StoreCarriedRows(T* st, int unit, const T* buf, int ld, int row0, const int* active) {
+  for (int i = (int)threadIdx.x; i < C * R * S; i += NT) {
+    const int c = i / (R * S), r = i % (R * S);
+    if (active[r % S]) st[unit * S + i] = buf[(size_t)c * ld + row0 * S + r];
+  }
+}
+
 // One fp32 residual unit:  d = dw(lrelu(u)); h = lrelu(pw1(d)); u' = pw2(h) + u.
 // u lives at row offset row0u of a [C][ldu] buffer; d is a [C][LDD] scratch.  When `last`, lrelu(u') is stored.
 // TC (decoder tensor-core mode): the two 1x1 convolutions run as split-precision TF32 MMAs with warp tiles of
@@ -114,8 +135,7 @@ template <int S, int NT, int TM, int TN1, int TN2, int WM, int KC, int C, int T,
           int WTM = 1, int WTN = 1, int STG = kStages>
 __device__ __forceinline__ void ResUnitF32(const uint8_t* blob, const ResF32& p, float* u, int ldu, int row0u, float* d,
                                            int groups2, float* ring, const int* n18,
-                                           const int* active, float* wbuf, bool last, const WNext& after, int pk, int& ph,
-                                           int dil_rt = DIL) {
+                                           const int* active, float* wbuf, bool last, const WNext& after, int dil_rt = DIL) {
   constexpr int ldd = LDD;
   // pw1's weight stream is started by whoever ran before this unit (previous GEMM or the kernel prologue)
   if (n18[S] >= 0) {
@@ -129,7 +149,6 @@ __device__ __forceinline__ void ResUnitF32(const uint8_t* blob, const ResF32& p,
   } else {
     DwF32Ring<S, NT>(u, ldu, row0u, d, ldd, C, T, dil_rt, BlobPtr<float>(blob, p.dw.w), BlobPtr<float>(blob, p.dw.bias), ring, n18, active);
   }
-  LYRA_PHASE(pk, ph);
   {
     const float* b1 = BlobPtr<float>(blob, p.pw1.bias);
     auto epi1 = [&](int t, int s0, int n0, auto& acc) {
@@ -148,7 +167,6 @@ __device__ __forceinline__ void ResUnitF32(const uint8_t* blob, const ResF32& p,
       GemmF32Tap<S, NT, TM, TN1, KC, WM, false, STG>(d, ldd, 0, 1, 1, C, 1, T, C, BlobPtr<float>(blob, p.pw1.w), wbuf, true,
                                                      NextF32(BlobPtr<float>(blob, p.pw2.w), KC, C, C / groups2, nullptr, STG), epi1);
   }
-  LYRA_PHASE(pk, ph);
   {
     const float* b2 = BlobPtr<float>(blob, p.pw2.bias);
     auto epi2 = [&](int t, int s0, int n0, auto& acc) {
@@ -169,7 +187,6 @@ __device__ __forceinline__ void ResUnitF32(const uint8_t* blob, const ResF32& p,
     else
       GemmF32Tap<S, NT, TM, TN2, KC, WM, false, STG>(d, ldd, 0, 1, 1, C / groups2, groups2, T, C, BlobPtr<float>(blob, p.pw2.w), wbuf, true, after, epi2);
   }
-  LYRA_PHASE(pk, ph);
 }
 
 // The three residual units of one stage (dilation 1, 3, 9; ring blocks of 2, 6, 18 rows back to back) as ONE copy of the code in
@@ -178,8 +195,7 @@ __device__ __forceinline__ void ResUnitF32(const uint8_t* blob, const ResF32& p,
 template <int S, int NT, int TM, int TN1, int TN2, int WM, int KC, int C, int T, bool TC = false, int LDD = T * S, int WTM = 1, int WTN = 1,
           int STG = kStages>
 __device__ __forceinline__ void ResUnitsF32x3(const uint8_t* blob, const ResF32* p3, float* u, int ldu, int row0u, float* d, int groups2,
-                                              float* ring0, const int* n18, const int* active, float* wbuf, const WNext& after,
-                                              int pk, int& ph) {
+                                              float* ring0, const int* n18, const int* active, float* wbuf, const WNext& after) {
 #pragma unroll 1
   for (int i = 0; i < 3; ++i) {
     const ResF32& p = p3[i];
@@ -187,8 +203,56 @@ __device__ __forceinline__ void ResUnitsF32x3(const uint8_t* blob, const ResF32*
     float* ring = ring0 + (size_t)(i == 0 ? 0 : (i == 1 ? 2 : 8)) * C * S;       // [C][2] | [C][6] | [C][18]
     const WNext nx = i < 2 ? NextF32(BlobPtr<float>(blob, p3[i + 1].pw1.w), KC, C, C, nullptr, STG) : after;
     ResUnitF32<S, NT, TM, TN1, TN2, WM, KC, C, T, 0, TC, LDD, WTM, WTN, STG>(blob, p, u, ldu, row0u, d, groups2, ring, n18, active, wbuf, i == 2, nx,
-                                                                       pk, ph, dil);
+                                                                       dil);
   }
+}
+
+// int8 GEMM epilogue: requantise the four channels n0 .. n0 + 3 of an accumulator, int8 LeakyReLU (lut), pack them into one word
+struct RequantLutPack {
+  const int* bias;
+  const int* mult;
+  const int* shift;
+  const int8_t* lut;
+  int out_zp;
+  __device__ __forceinline__ RequantLutPack(const uint8_t* blob, const GemmI8& g, const LReluQ& lr)
+      : bias(BlobPtr<int>(blob, g.bias)), mult(BlobPtr<int>(blob, g.mult)), shift(BlobPtr<int>(blob, g.shift)),
+        lut(BlobPtr<int8_t>(blob, lr.lut)), out_zp(g.out_zp) {}
+  __device__ __forceinline__ uint32_t operator()(const int (&acc)[1][4], int n0) const {
+    const RequantP4 rq = LoadRequant4(bias, mult, shift, n0);
+    int q[4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) q[j] = lut[RequantI8(acc[0][j], rq.b[j], rq.m[j], rq.s[j], out_zp) + 128];
+    return PackI8x4(q[0], q[1], q[2], q[3]);
+  }
+};
+
+// The int8 half of the mixed residual unit (encoder_2/resnet_0, quant_decoder_0/resnet_0): its second 1x1 convolution (4 groups)
+// on hq, DEQUANTIZE + the f32 residual u [256][2S], QUANTIZE -> resq, int8 LeakyReLU -> aq rows row0a, row0a + 1.
+// P: EncoderParams or DecoderParams (the same m_pw2 / m_dq / m_q2 / m_lr2 fields).
+template <int S, int NT, int PDI, typename Params>
+__device__ __forceinline__ void MixedUnitPw2I8(const uint8_t* blob, const Params& P, const uint32_t* hq, const float* u,
+                                               uint32_t* resq, uint32_t* aq, int lda, int row0a) {
+  constexpr int LQ2 = PadLd(2 * S), LD2 = 2 * S;
+  const int* bias = BlobPtr<int>(blob, P.m_pw2.bias);
+  const int* mult = BlobPtr<int>(blob, P.m_pw2.mult);
+  const int* shift = BlobPtr<int>(blob, P.m_pw2.shift);
+  const int8_t* lut = BlobPtr<int8_t>(blob, P.m_lr2.lut);
+  const QuantP dq = P.m_dq, q2 = P.m_q2;
+  const int out_zp = P.m_pw2.out_zp;
+  GemmI8Mma<S, NT, 4, PDI>(hq, LQ2, 0, 1, 1, 64, 4, 2, 256, BlobPtr<uint2>(blob, P.m_pw2.w),
+    [&](int t, int s, int n0, int (&acc)[1][4]) {
+      const RequantP4 rq = LoadRequant4(bias, mult, shift, n0);
+      int r[4], a[4];
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const int q = RequantI8(acc[0][j], rq.b[j], rq.m[j], rq.s[j], out_zp);
+        const float v = __fadd_rn(DequantizeI8(q, dq.scale, dq.zp), u[(size_t)(n0 + j) * LD2 + t * S + s]);
+        r[j] = QuantizeF32(v, q2.scale, q2.zp);
+        a[j] = lut[r[j] + 128];
+      }
+      resq[(size_t)(n0 / 4) * LQ2 + t * S + s] = PackI8x4(r[0], r[1], r[2], r[3]);
+      aq[(size_t)(n0 / 4) * lda + (row0a + t) * S + s] = PackI8x4(a[0], a[1], a[2], a[3]);
+    });
 }
 
 // One int8 residual unit on packed activations (quant_encoder_2/resnet_{1,2}, quant_decoder_0/resnet_{1,2}); the two
@@ -197,7 +261,7 @@ __device__ __forceinline__ void ResUnitsF32x3(const uint8_t* blob, const ResF32*
 template <int S, int NT, int DIL, int PDI = kI8Pd>
 __device__ __forceinline__ void ResUnitI8(const uint8_t* blob, const ResI8& p, uint32_t* aq, int lda, int row0a,
                                           uint32_t* resq, uint32_t* dq8, uint32_t* hq, uint32_t* ring,
-                                          const int* n18, const int* active, int pk, int& ph, int dil_rt = DIL) {
+                                          const int* n18, const int* active, int dil_rt = DIL) {
   constexpr int T = 2, C = 256, LD = PadLd(T * S);
   constexpr int NTW = 4;
   if (n18[S] >= 0) {
@@ -207,23 +271,11 @@ __device__ __forceinline__ void ResUnitI8(const uint8_t* blob, const ResI8& p, u
   } else {
     DwI8Ring<S, NT>(aq, lda, row0a, dq8, LD, C, T, dil_rt, blob, p.dw, ring, n18, active);
   }
-  LYRA_PHASE(pk, ph);
   {
-    const int* bias = BlobPtr<int>(blob, p.pw1.bias);
-    const int* mult = BlobPtr<int>(blob, p.pw1.mult);
-    const int* shift = BlobPtr<int>(blob, p.pw1.shift);
-    const int8_t* lut = BlobPtr<int8_t>(blob, p.lr1.lut);
-    const int out_zp = p.pw1.out_zp;
+    const RequantLutPack epi(blob, p.pw1, p.lr1);
     GemmI8Mma<S, NT, NTW, PDI>(dq8, LD, 0, 1, 1, C, 1, T, C, BlobPtr<uint2>(blob, p.pw1.w),
-      [&](int t, int s, int n0, int (&acc)[1][4]) {
-        const RequantP4 rq = LoadRequant4(bias, mult, shift, n0);
-        int q[4];
-#pragma unroll
-        for (int j = 0; j < 4; ++j) q[j] = lut[RequantI8(acc[0][j], rq.b[j], rq.m[j], rq.s[j], out_zp) + 128];
-        hq[(size_t)(n0 / 4) * LD + t * S + s] = PackI8x4(q[0], q[1], q[2], q[3]);
-      });
+      [&](int t, int s, int n0, int (&acc)[1][4]) { hq[(size_t)(n0 / 4) * LD + t * S + s] = epi(acc, n0); });
   }
-  LYRA_PHASE(pk, ph);
   {
     const int* bias = BlobPtr<int>(blob, p.pw2.bias);
     const int* mult = BlobPtr<int>(blob, p.pw2.mult);
@@ -248,17 +300,16 @@ __device__ __forceinline__ void ResUnitI8(const uint8_t* blob, const ResI8& p, u
         aq[(size_t)(n0 / 4) * lda + (row0a + t) * S + s] = PackI8x4(a[0], a[1], a[2], a[3]);
       });
   }
-  LYRA_PHASE(pk, ph);
 }
 
 // quant_{en,de}coder resnet_1 and resnet_2 (dilation 3, 9; ring blocks of 6 and 18 rows back to back) as one copy of the code
 template <int S, int NT, int PDI = kI8Pd>
 __device__ __forceinline__ void ResUnitsI8x2(const uint8_t* blob, const ResI8* p2, uint32_t* aq, int lda, int row0a,
                                              uint32_t* resq, uint32_t* dq8, uint32_t* hq, uint32_t* ring0,
-                                             const int* n18, const int* active, int pk, int& ph) {
+                                             const int* n18, const int* active) {
 #pragma unroll 1
   for (int i = 0; i < 2; ++i)
-    ResUnitI8<S, NT, 0, PDI>(blob, p2[i], aq, lda, row0a, resq, dq8, hq, ring0 + (size_t)(i ? 64 * 6 : 0) * S, n18, active, pk, ph, i ? 9 : 3);
+    ResUnitI8<S, NT, 0, PDI>(blob, p2[i], aq, lda, row0a, resq, dq8, hq, ring0 + (size_t)(i ? 64 * 6 : 0) * S, n18, active, i ? 9 : 3);
 }
 
 // ================================================================================================
@@ -296,14 +347,10 @@ EncoderKernelA(const uint8_t* __restrict__ blob, EncoderParams P, TileIo io, con
   int* n18 = active + S;
   int tile;
   InitWeightPipe<NT>();
-  LoadTileMeta<S>(io, n18g, slot, active, n18, tile);
-  if (n18[S] == kTileIdle) return;
+  if (!BeginTile<S>(io, n18g, slot, state, EncStateA::kUnits, tile)) return;
   float* st = state + (size_t)tile * EncStateA::kUnits * S;
   const int tid = (int)threadIdx.x;
-  PrefetchTileState(st, EncStateA::kUnits * S * 4);
   IssuePrologue<NT>(wbuf, NextF32(BlobPtr<float>(blob, P.first.w), 16, 64, 64));
-  int ph = 0;
-  LYRA_PHASE(0, ph);
 
   // ---- input window X[368][S] (aliases d): 48 carried samples + 320 new ones as unit floats (dsp_utils.h:104-108)
   float* X = d;
@@ -320,7 +367,6 @@ EncoderKernelA(const uint8_t* __restrict__ blob, EncoderParams P, TileIo io, con
   __syncthreads();
   for (int i = tid; i < 48 * S; i += NT)
     if (active[i % S]) { const int r = 320 + i / S; st[EncStateA::kFirst * S + i] = X[(r + (r >> 4)) * S + i % S]; }
-  LYRA_PHASE(0, ph);
   // ---- first_layer: K = 64, stride 16, 1 -> 64 ; u = conv + bias (pre-activation residual stream)
   {
     const float* b = BlobPtr<float>(blob, P.first.bias);
@@ -336,17 +382,12 @@ EncoderKernelA(const uint8_t* __restrict__ blob, EncoderParams P, TileIo io, con
       });
   }
   // ---- encoder_0: three residual units, dilation 1/3/9
-  LYRA_PHASE(0, ph);
   static_assert(EncStateA::kRing1 == EncStateA::kRing0 + 64 * 2 && EncStateA::kRing2 == EncStateA::kRing1 + 64 * 6, "ring blocks back to back");
   ResUnitsF32x3<S, NT, 8, L::TN, L::TN, 4, 16, 64, 20>(blob, P.r0, u, L::LDU, 5, d, 1, st + (size_t)EncStateA::kRing0 * S, n18, active, wbuf,
-                                                       NextF32(BlobPtr<float>(blob, P.down0.w), 16, 128, 640, d, L::kStgDown), 0, ph);
+                                                       NextF32(BlobPtr<float>(blob, P.down0.w), 16, 128, 640, d, L::kStgDown));
   // carried rows for the next frame: the last 5 activated rows
-  for (int i = tid; i < 64 * 5 * S; i += NT) {
-    const int c = i / (5 * S), r = i % (5 * S);
-    if (active[r % S]) st[EncStateA::kDown0 * S + i] = u[(size_t)c * L::LDU + 20 * S + r];
-  }
+  StoreCarriedRows<S, NT, 64, 5>(st, EncStateA::kDown0, u, L::LDU, 20, active);
   // ---- encoder_0/simpleconv: K = 10, stride 5, 64 -> 128 ; pre-activation output to HBM for kernel B
-  LYRA_PHASE(0, ph);
   {
     const float* b = BlobPtr<float>(blob, P.down0.bias);
     float* out = mid + (size_t)tile * 128 * 4 * S;
@@ -364,8 +405,7 @@ EncoderKernelA(const uint8_t* __restrict__ blob, EncoderParams P, TileIo io, con
         }
       });
   }
-  if (tid < S && active[tid]) n18g[tile * S + tid] = (n18[tid] + 1) % 18;
-  LYRA_PHASE(0, ph);
+  AdvanceHopCounters<S>(n18g, tile, active, n18);
 }
 
 // ================================================================================================
@@ -425,15 +465,10 @@ EncoderKernelB(const uint8_t* __restrict__ blob, EncoderParams P, TileIo io, con
   int* n18 = active + S;
   int tile;
   InitWeightPipe<NT>();
-  LoadTileMeta<S>(io, n18g, slot, active, n18, tile);
-  if (n18[S] == kTileIdle) return;
-  uint32_t* stw = reinterpret_cast<uint32_t*>(state) + (size_t)tile * EncStateB::kUnits * S;
-  float* st = reinterpret_cast<float*>(stw);
-  const int tid = (int)threadIdx.x;
-  PrefetchTileState(st, EncStateB::kUnits * S * 4);
+  if (!BeginTile<S>(io, n18g, slot, state, EncStateB::kUnits, tile)) return;
+  float* st = state + (size_t)tile * EncStateB::kUnits * S;
+  uint32_t* stw = reinterpret_cast<uint32_t*>(st);
   IssuePrologue<NT>(wbuf, NextF32(BlobPtr<float>(blob, P.r1[0].pw1.w), 16, 128, 128, nullptr, L::kStg));
-  int ph = 0;
-  LYRA_PHASE(1, ph);
 
   // ---- u1 <- kernel A output (rows 2..5), carried rows of encoder_1/simpleconv (rows 0..1)
   {
@@ -445,17 +480,12 @@ EncoderKernelB(const uint8_t* __restrict__ blob, EncoderParams P, TileIo io, con
   }
   __syncthreads();
   // ---- encoder_1: three residual units @128 (second 1x1 has 2 groups)
-  LYRA_PHASE(1, ph);
   static_assert(EncStateB::kRing1 == EncStateB::kRing0 + 128 * 2 && EncStateB::kRing2 == EncStateB::kRing1 + 128 * 6, "ring blocks back to back");
   ResUnitsF32x3<S, NT, TM, TN, TN, L::WM4, 16, 128, 4, false, 4 * S, 1, 1, L::kStg>(
       blob, P.r1, u1, L::LD1, 2, d1, 2, st + (size_t)EncStateB::kRing0 * S, n18, active, wbuf,
-      NextF32(BlobPtr<float>(blob, P.down1.w), 8, 256, 256, wbuf, L::kStg), 1, ph);
-  for (int i = tid; i < 128 * 2 * S; i += NT) {
-    const int c = i / (2 * S), r = i % (2 * S);
-    if (active[r % S]) st[EncStateB::kDown1 * S + i] = u1[(size_t)c * L::LD1 + 4 * S + r];
-  }
+      NextF32(BlobPtr<float>(blob, P.down1.w), 8, 256, 256, wbuf, L::kStg));
+  StoreCarriedRows<S, NT, 128, 2>(st, EncStateB::kDown1, u1, L::LD1, 4, active);
   // ---- encoder_1/simpleconv: K = 4, stride 2, 128 -> 256, 2 groups ; u2 = pre-activation
-  LYRA_PHASE(1, ph);
   {
     const float* b = BlobPtr<float>(blob, P.down1.bias);
     GemmF32Tap<S, NT, TM, TN, 8, L::WM2, false, L::kStg>(u1, L::LD1, 0, 2, 4, 64, 2, 2, 256, BlobPtr<float>(blob, P.down1.w), wbuf, true,
@@ -472,7 +502,6 @@ EncoderKernelB(const uint8_t* __restrict__ blob, EncoderParams P, TileIo io, con
   // ---- encoder_2/resnet_0 (mixed): f32 depthwise + f32 1x1, QUANTIZE, int8 LeakyReLU, int8 1x1 (4 groups),
   //      DEQUANTIZE + f32 residual, QUANTIZE, int8 LeakyReLU
   constexpr int LD2 = 2 * S;
-  LYRA_PHASE(1, ph);
   if (n18[S] >= 0)
     DwF32RingFast<S, NT, 256, 2, 1>(u2, LD2, 0, d2, LD2, BlobPtr<float>(blob, P.m_dw.w), BlobPtr<float>(blob, P.m_dw.bias),
                                     st + (size_t)EncStateB::kRingM * S, n18[S], active);
@@ -497,66 +526,25 @@ EncoderKernelB(const uint8_t* __restrict__ blob, EncoderParams P, TileIo io, con
         }
       });
   }
-  {
-    const int* bias = BlobPtr<int>(blob, P.m_pw2.bias);
-    const int* mult = BlobPtr<int>(blob, P.m_pw2.mult);
-    const int* shift = BlobPtr<int>(blob, P.m_pw2.shift);
-    const int8_t* lut = BlobPtr<int8_t>(blob, P.m_lr2.lut);
-    const QuantP dq = P.m_dq, q2 = P.m_q2;
-    const int out_zp = P.m_pw2.out_zp;
-    GemmI8Mma<S, NT, 4, L::kI8Pd>(hq, LQ2, 0, 1, 1, 64, 4, 2, 256, BlobPtr<uint2>(blob, P.m_pw2.w),
-      [&](int t, int s, int n0, int (&acc)[1][4]) {
-        const RequantP4 rq = LoadRequant4(bias, mult, shift, n0);
-        int r[4], a[4];
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const int q = RequantI8(acc[0][j], rq.b[j], rq.m[j], rq.s[j], out_zp);
-          const float v = __fadd_rn(DequantizeI8(q, dq.scale, dq.zp), u2[(size_t)(n0 + j) * LD2 + t * S + s]);
-          r[j] = QuantizeF32(v, q2.scale, q2.zp);
-          a[j] = lut[r[j] + 128];
-        }
-        resq[(size_t)(n0 / 4) * LQ2 + t * S + s] = PackI8x4(r[0], r[1], r[2], r[3]);
-        aq[(size_t)(n0 / 4) * LQA + (2 + t) * S + s] = PackI8x4(a[0], a[1], a[2], a[3]);
-      });
-  }
+  MixedUnitPw2I8<S, NT, L::kI8Pd>(blob, P, hq, u2, resq, aq, LQA, 2);
   // ---- quant_encoder_2/resnet_{1,2}
-  LYRA_PHASE(1, ph);
   static_assert(EncStateB::kRingQ1 == EncStateB::kRingQ0 + 64 * 6, "ring blocks back to back");
-  ResUnitsI8x2<S, NT, L::kI8Pd>(blob, P.q, aq, LQA, 2, resq, dq8, hq, stw + (size_t)EncStateB::kRingQ0 * S, n18, active, 1, ph);
+  ResUnitsI8x2<S, NT, L::kI8Pd>(blob, P.q, aq, LQA, 2, resq, dq8, hq, stw + (size_t)EncStateB::kRingQ0 * S, n18, active);
   // ---- quant_encoder_2/simpleconv: K = 4, stride 2, 256 -> 512, 4 groups, then int8 LeakyReLU
-  LYRA_PHASE(1, ph);
   BatchedLoop<NT, 4, uint32_t>(64 * 2 * S, [&](int i) { return stw[EncStateB::kDown2 * S + i]; },
     [&](int i, uint32_t v) { const int c = i / (2 * S), r = i % (2 * S); aq[(size_t)c * LQA + r] = v; });
   BatchedLoop<NT, 8, uint32_t>(128 * 2 * S, [&](int i) { return stw[EncStateB::kBott * S + i]; },
     [&](int i, uint32_t v) { const int c = i / (2 * S), r = i % (2 * S); bq[(size_t)c * LQB + r] = v; });
   __syncthreads();
-  for (int i = tid; i < 64 * 2 * S; i += NT) {
-    const int c = i / (2 * S), r = i % (2 * S);
-    if (active[r % S]) stw[EncStateB::kDown2 * S + i] = aq[(size_t)c * LQA + 2 * S + r];
-  }
+  StoreCarriedRows<S, NT, 64, 2>(stw, EncStateB::kDown2, aq, LQA, 2, active);
   {
-    const int* bias = BlobPtr<int>(blob, P.down2.bias);
-    const int* mult = BlobPtr<int>(blob, P.down2.mult);
-    const int* shift = BlobPtr<int>(blob, P.down2.shift);
-    const int8_t* lut = BlobPtr<int8_t>(blob, P.down2_lr.lut);
-    const int out_zp = P.down2.out_zp;
+    const RequantLutPack epi(blob, P.down2, P.down2_lr);
     GemmI8Mma<S, NT, 8, L::kI8Pd>(aq, LQA, 0, 2, 4, 64, 4, 1, 512, BlobPtr<uint2>(blob, P.down2.w),
-      [&](int t, int s, int n0, int (&acc)[1][4]) {
-        const RequantP4 rq = LoadRequant4(bias, mult, shift, n0);
-        (void)t;
-        int q[4];
-#pragma unroll
-        for (int j = 0; j < 4; ++j) q[j] = lut[RequantI8(acc[0][j], rq.b[j], rq.m[j], rq.s[j], out_zp) + 128];
-        bq[(size_t)(n0 / 4) * LQB + 2 * S + s] = PackI8x4(q[0], q[1], q[2], q[3]);
-      });
+      [&](int, int s, int n0, int (&acc)[1][4]) { bq[(size_t)(n0 / 4) * LQB + 2 * S + s] = epi(acc, n0); });
   }
   // carried rows of quant_bottleneck_1: the two newest rows
-  for (int i = tid; i < 128 * 2 * S; i += NT) {
-    const int c = i / (2 * S), r = i % (2 * S);
-    if (active[r % S]) stw[EncStateB::kBott * S + i] = bq[(size_t)c * LQB + S + r];
-  }
+  StoreCarriedRows<S, NT, 128, 2>(stw, EncStateB::kBott, bq, LQB, 1, active);
   // ---- quant_bottleneck_1: K = 3, 512 -> 64, 4 groups ; DEQUANTIZE -> features
-  LYRA_PHASE(1, ph);
   {
     const int* bias = BlobPtr<int>(blob, P.bott.bias);
     const int* mult = BlobPtr<int>(blob, P.bott.mult);
@@ -574,8 +562,7 @@ EncoderKernelB(const uint8_t* __restrict__ blob, EncoderParams P, TileIo io, con
           o[j] = DequantizeI8(RequantI8(acc[0][j], rq.b[j], rq.m[j], rq.s[j], out_zp), dq.scale, dq.zp);
       });
   }
-  if (tid < S && active[tid]) n18g[tile * S + tid] = (n18[tid] + 1) % 18;
-  LYRA_PHASE(1, ph);
+  AdvanceHopCounters<S>(n18g, tile, active, n18);
 }
 
 // ================================================================================================
@@ -637,18 +624,14 @@ DecoderKernelC(const uint8_t* __restrict__ blob, DecoderParams P, TileIo io,
   int* n18 = active + S;
   int tile;
   InitWeightPipe<NT>();
-  LoadTileMeta<S>(io, n18g, slot, active, n18, tile);
-  if (n18[S] == kTileIdle) return;
+  if (!BeginTile<S>(io, n18g, slot, state, DecStateC::kUnits, tile)) return;
   uint32_t* stw = reinterpret_cast<uint32_t*>(state) + (size_t)tile * DecStateC::kUnits * S;
   float* st = reinterpret_cast<float*>(stw);
   const int tid = (int)threadIdx.x;
-  PrefetchTileState(st, DecStateC::kUnits * S * 4);
   constexpr int LD2 = 2 * S;
   const UpI8& up0 = P.up0;
   const UpI8& up1 = P.up1;
   IssuePrologue<NT>(wbuf, NextF32(BlobPtr<float>(blob, P.bott.w), 4, 512, 48));
-  int ph = 0;
-  LYRA_PHASE(2, ph);
 
   // ---- F: 2 carried feature rows + the new one ; overlap states into u ; padding rows of xq
   BatchedLoop<NT, 4, float>(64 * 2 * S, [&](int i) { return st[DecStateC::kBott * S + i]; },
@@ -662,12 +645,8 @@ DecoderKernelC(const uint8_t* __restrict__ blob, DecoderParams P, TileIo io,
     for (int i = tid; i < 128 * S; i += NT) { const int c = i / S, s = i % S; xq[(size_t)c * LQB + s] = pad; xq[(size_t)c * LQB + 2 * S + s] = pad; }
   }
   __syncthreads();
-  for (int i = tid; i < 64 * 2 * S; i += NT) {
-    const int c = i / (2 * S), r = i % (2 * S);
-    if (active[r % S]) st[DecStateC::kBott * S + i] = F[(size_t)c * 3 * S + S + r];
-  }
+  StoreCarriedRows<S, NT, 64, 2>(st, DecStateC::kBott, F, 3 * S, 1, active);
   // ---- bottleneck_2/simpleconv: K = 3, 64 -> 512, 4 groups ; LeakyReLU ; QUANTIZE
-  LYRA_PHASE(2, ph);
   {
     const float* b = BlobPtr<float>(blob, P.bott.bias);
     const QuantP q = P.bott_q;
@@ -685,7 +664,6 @@ DecoderKernelC(const uint8_t* __restrict__ blob, DecoderParams P, TileIo io,
       });
   }
   // ---- quant_decoder_0 upsample: 4 x TRANSPOSE_CONV (K = 4, stride 2, 128 -> 64), T 1 -> 2 (+2 tail rows)
-  LYRA_PHASE(2, ph);
   {
     const int* bias = BlobPtr<int>(blob, up0.g.bias);
     const int* mult = BlobPtr<int>(blob, up0.g.mult);
@@ -711,7 +689,6 @@ DecoderKernelC(const uint8_t* __restrict__ blob, DecoderParams P, TileIo io,
       });
   }
   // ---- LeakyReLU (f32) ; QUANTIZE -> aq rows 1..2
-  LYRA_PHASE(2, ph);
   {
     const QuantP q = P.up0_q;
     for (int i = tid; i < 64 * 2 * S; i += NT) {
@@ -724,51 +701,17 @@ DecoderKernelC(const uint8_t* __restrict__ blob, DecoderParams P, TileIo io,
   }
   __syncthreads();
   // ---- quant_decoder_0/resnet_0 (int8 body, f32 residual add)
-  LYRA_PHASE(2, ph);
   if (n18[S] >= 0) DwI8RingFast<S, NT, 256, 2, 1>(aq, LQA, 1, dq8, LQ2, blob, P.m_dw, stw + (size_t)DecStateC::kRingM * S, n18[S], active);
   else DwI8Ring<S, NT>(aq, LQA, 1, dq8, LQ2, 256, 2, 1, blob, P.m_dw, stw + (size_t)DecStateC::kRingM * S, n18, active);
   {
-    const int* bias = BlobPtr<int>(blob, P.m_pw1.bias);
-    const int* mult = BlobPtr<int>(blob, P.m_pw1.mult);
-    const int* shift = BlobPtr<int>(blob, P.m_pw1.shift);
-    const int8_t* lut = BlobPtr<int8_t>(blob, P.m_lr1.lut);
-    const int out_zp = P.m_pw1.out_zp;
+    const RequantLutPack epi(blob, P.m_pw1, P.m_lr1);
     GemmI8Mma<S, NT, 4, L::kI8Pd>(dq8, LQ2, 0, 1, 1, 256, 1, 2, 256, BlobPtr<uint2>(blob, P.m_pw1.w),
-      [&](int t, int s, int n0, int (&acc)[1][4]) {
-        const RequantP4 rq = LoadRequant4(bias, mult, shift, n0);
-        int q[4];
-#pragma unroll
-        for (int j = 0; j < 4; ++j) q[j] = lut[RequantI8(acc[0][j], rq.b[j], rq.m[j], rq.s[j], out_zp) + 128];
-        hq[(size_t)(n0 / 4) * LQ2 + t * S + s] = PackI8x4(q[0], q[1], q[2], q[3]);
-      });
+      [&](int t, int s, int n0, int (&acc)[1][4]) { hq[(size_t)(n0 / 4) * LQ2 + t * S + s] = epi(acc, n0); });
   }
-  {
-    const int* bias = BlobPtr<int>(blob, P.m_pw2.bias);
-    const int* mult = BlobPtr<int>(blob, P.m_pw2.mult);
-    const int* shift = BlobPtr<int>(blob, P.m_pw2.shift);
-    const int8_t* lut = BlobPtr<int8_t>(blob, P.m_lr2.lut);
-    const QuantP dq = P.m_dq, q2 = P.m_q2;
-    const int out_zp = P.m_pw2.out_zp;
-    GemmI8Mma<S, NT, 4, L::kI8Pd>(hq, LQ2, 0, 1, 1, 64, 4, 2, 256, BlobPtr<uint2>(blob, P.m_pw2.w),
-      [&](int t, int s, int n0, int (&acc)[1][4]) {
-        const RequantP4 rq = LoadRequant4(bias, mult, shift, n0);
-        int r[4], a[4];
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const int q = RequantI8(acc[0][j], rq.b[j], rq.m[j], rq.s[j], out_zp);
-          const float v = __fadd_rn(DequantizeI8(q, dq.scale, dq.zp), u[(size_t)(n0 + j) * LD2 + t * S + s]);
-          r[j] = QuantizeF32(v, q2.scale, q2.zp);
-          a[j] = lut[r[j] + 128];
-        }
-        resq[(size_t)(n0 / 4) * LQ2 + t * S + s] = PackI8x4(r[0], r[1], r[2], r[3]);
-        aq[(size_t)(n0 / 4) * LQA + (1 + t) * S + s] = PackI8x4(a[0], a[1], a[2], a[3]);
-      });
-  }
-  LYRA_PHASE(2, ph);
+  MixedUnitPw2I8<S, NT, L::kI8Pd>(blob, P, hq, u, resq, aq, LQA, 1);
   static_assert(DecStateC::kRingQ1 == DecStateC::kRingQ0 + 64 * 6, "ring blocks back to back");
-  ResUnitsI8x2<S, NT, L::kI8Pd>(blob, P.q, aq, LQA, 1, resq, dq8, hq, stw + (size_t)DecStateC::kRingQ0 * S, n18, active, 2, ph);
+  ResUnitsI8x2<S, NT, L::kI8Pd>(blob, P.q, aq, LQA, 1, resq, dq8, hq, stw + (size_t)DecStateC::kRingQ0 * S, n18, active);
   // ---- quant_decoder_1 upsample: 2 x TRANSPOSE_CONV (K = 4, stride 2, 128 -> 64), T 2 -> 4 (+2 tail rows)
-  LYRA_PHASE(2, ph);
   {
     const uint32_t pad = PackI8x4(up1.g.in_zp, up1.g.in_zp, up1.g.in_zp, up1.g.in_zp);
     for (int i = tid; i < 64 * S; i += NT) { const int c = i / S, s = i % S; aq[(size_t)c * LQA + s] = pad; aq[(size_t)c * LQA + 3 * S + s] = pad; }
@@ -804,16 +747,14 @@ DecoderKernelC(const uint8_t* __restrict__ blob, DecoderParams P, TileIo io,
       });
   }
   // ---- decoder_1: three fp32 residual units @128
-  LYRA_PHASE(2, ph);
   static_assert(DecStateC::kRing1 == DecStateC::kRing0 + 128 * 2 && DecStateC::kRing2 == DecStateC::kRing1 + 128 * 6, "ring blocks back to back");
   ResUnitsF32x3<S, NT, TM, TN, TN, L::WM4, 16, 128, 4, TC, L::LD1, L::RWM, L::RWN>(
-      blob, P.r1, u1, 4 * S, 0, d1, 2, st + (size_t)DecStateC::kRing0 * S, n18, active, wbuf, NoNext(), 2, ph);
+      blob, P.r1, u1, 4 * S, 0, d1, 2, st + (size_t)DecStateC::kRing0 * S, n18, active, wbuf, NoNext());
   {
     float* out = mid + (size_t)tile * 128 * 4 * S;
     for (int i = tid; i < 128 * 4 * S; i += NT) out[i] = u1[i];
   }
-  if (tid < S && active[tid]) n18g[tile * S + tid] = (n18[tid] + 1) % 18;
-  LYRA_PHASE(2, ph);
+  AdvanceHopCounters<S>(n18g, tile, active, n18);
 }
 
 // ================================================================================================
@@ -860,16 +801,12 @@ DecoderKernelD(const uint8_t* __restrict__ blob, DecoderParams P, TileIo io, con
   int* n18 = active + S;
   int tile;
   InitWeightPipe<NT>();
-  LoadTileMeta<S>(io, n18g, slot, active, n18, tile);
-  if (n18[S] == kTileIdle) return;
+  if (!BeginTile<S>(io, n18g, slot, state, DecStateD::kUnits, tile)) return;
   float* st = state + (size_t)tile * DecStateD::kUnits * S;
   const int tid = (int)threadIdx.x;
-  PrefetchTileState(st, DecStateD::kUnits * S * 4);
   constexpr int LDX = L::LDX;
   float* wbuf_up2 = X + 128 * LDX;       // free tail of d + the regular ring
   IssuePrologue<NT>(wbuf_up2, NextF32(BlobPtr<float>(blob, P.up2.w), L::KCU, 320, 256));
-  int ph = 0;
-  LYRA_PHASE(3, ph);
 
   // ---- X [128][6S]: zero row, 4 rows from kernel C, zero row
   {
@@ -888,7 +825,6 @@ DecoderKernelD(const uint8_t* __restrict__ blob, DecoderParams P, TileIo io, con
   }
   __syncthreads();
   // ---- decoder_2/simple: TRANSPOSE_CONV K = 10, stride 5, 128 -> 64 ; T 4 -> 20 (+5 tail rows)
-  LYRA_PHASE(3, ph);
   {
     const float* b = BlobPtr<float>(blob, P.up2.bias);
     float* tail = st + (size_t)DecStateD::kUp2 * S;
@@ -914,12 +850,10 @@ DecoderKernelD(const uint8_t* __restrict__ blob, DecoderParams P, TileIo io, con
                                                         NextF32(BlobPtr<float>(blob, P.r2[0].pw1.w), 16, 64, 64, wbuf), epi_up);
   }
   // ---- decoder_2: three residual units @64, T = 20
-  LYRA_PHASE(3, ph);
   static_assert(DecStateD::kRing1 == DecStateD::kRing0 + 64 * 2 && DecStateD::kRing2 == DecStateD::kRing1 + 64 * 6, "ring blocks back to back");
   ResUnitsF32x3<S, NT, 8, L::TN, L::TN, 4, 16, 64, 20>(blob, P.r2, u, L::LDU, 3, d, 1, st + (size_t)DecStateD::kRing0 * S, n18, active, wbuf,
-                                                       NextF32(BlobPtr<float>(blob, P.last.w), 16, 16, 256), 3, ph);
+                                                       NextF32(BlobPtr<float>(blob, P.last.w), 16, 16, 256));
   // ---- last_layer: TRANSPOSE_CONV K = 64, stride 16, 64 -> 1 ; T 20 -> 320 (+48 tail) ; float -> int16
-  LYRA_PHASE(3, ph);
   {
     const float bias = BlobPtr<float>(blob, P.last.bias)[0];
     float* tail = st + (size_t)DecStateD::kLast * S;
@@ -950,8 +884,7 @@ DecoderKernelD(const uint8_t* __restrict__ blob, DecoderParams P, TileIo io, con
       if (active[s]) pcm[(size_t)slot[s] * 320 + (i % 320)] = stage[i];
     }
   }
-  if (tid < S && active[tid]) n18g[tile * S + tid] = (n18[tid] + 1) % 18;
-  LYRA_PHASE(3, ph);
+  AdvanceHopCounters<S>(n18g, tile, active, n18);
 }
 
 }  // namespace lyra_b200

@@ -115,7 +115,7 @@ DecoderKernelDW(const uint8_t* __restrict__ blob, DecoderParams P, TileIo io, co
   float* slo = smf + L::kSlOut / 4;
   int* slot = reinterpret_cast<int*>(smem + L::kI);
   int* active = slot + S;
-  int* n18 = active + S;                                      // n18[S]: tile summary (LoadTileMeta)
+  int* n18 = active + S;                                      // n18[S]: tile summary (BeginTile)
   LYRA_STATIC_SMEM(DecDWShared, sh, 1);
   const int tid = (int)threadIdx.x, warp = tid >> 5, lane = tid & 31;
 
@@ -129,12 +129,12 @@ DecoderKernelDW(const uint8_t* __restrict__ blob, DecoderParams P, TileIo io, co
     for (int i = 0; i < 2; ++i) lyra_mbar_init(&sh->ring_full[i], 1);
     lyra_mbar_fence_init();
   }
+  // BeginTile holds two block barriers: the barrier inits above are visible after it.  Its L2 prefetch of the tile's state also
+  // serves unit 2, which reads its ring block from global memory.
   int tile;
-  LoadTileMeta<S>(io, n18g, slot, active, n18, tile);       // two block barriers inside: the barrier inits are visible after it
-  if (n18[S] == kTileIdle) return;
+  if (!BeginTile<S>(io, n18g, slot, state, DecStateD::kUnits, tile)) return;
   float* st = state + (size_t)tile * DecStateD::kUnits * S;
   const uint8_t* chunks = blob + P.du_chunks;
-  PrefetchTileState(st, DecStateD::kUnits * S * 4);                          // unit 2 reads its ring block from global memory
 
   // ================================================= TMA producer =================================================
   if (warp == L::kTmaWarp) {
@@ -417,7 +417,7 @@ DecoderKernelDW(const uint8_t* __restrict__ blob, DecoderParams P, TileIo io, co
     const int ss = (2 * i) / 320;
     if (active[ss]) *reinterpret_cast<uint32_t*>(pcm + (size_t)slot[ss] * 320 + (2 * i) % 320) = reinterpret_cast<const uint32_t*>(stage)[i];
   }
-  if (tid < S && active[tid]) n18g[tile * S + tid] = (n18[tid] + 1) % 18;
+  AdvanceHopCounters<S>(n18g, tile, active, n18);
   if (tid == 0) lyra_bulk_wait_all();                        // every state block is in global memory before the block exits
 }
 

@@ -57,31 +57,6 @@ __device__ __forceinline__ uint32_t CngPhaseIndex(unsigned long long seed, unsig
   return (uint32_t)(x >> 54);
 }
 
-// three consecutive inverse-transform stages: FftButterflies3 with conjugated twiddles
-template <int STRIDE>
-__device__ __forceinline__ void IfftButterflies3(double (&xr)[8], double (&xi)[8], int r, const double2* __restrict__ tw) {
-#pragma unroll
-  for (int s = 0; s < 3; ++s) {
-    const int half = STRIDE << s;
-#pragma unroll
-    for (int j = 0; j < 8; ++j)
-      if (!(j & (1 << s))) {
-        const int k = r + (j & ((1 << s) - 1)) * STRIDE;
-        const double2 w = tw[half - 1 + k];
-        FftButterfly(xr[j], xi[j], xr[j + (1 << s)], xi[j + (1 << s)], w.x, -w.y);
-      }
-  }
-}
-template <int STRIDE>
-__device__ __forceinline__ void IfftStages3(double* re, double* im, int base, int r, const double2* __restrict__ tw) {
-  double xr[8], xi[8];
-#pragma unroll
-  for (int j = 0; j < 8; ++j) { xr[j] = re[FftIdx(base + j * STRIDE)]; xi[j] = im[FftIdx(base + j * STRIDE)]; }
-  IfftButterflies3<STRIDE>(xr, xi, r, tw);
-#pragma unroll
-  for (int j = 0; j < 8; ++j) { re[FftIdx(base + j * STRIDE)] = xr[j]; im[FftIdx(base + j * STRIDE)] = xi[j]; }
-}
-
 // One block of 128 threads per stream.  features: [n][160] conditioning log-mel vectors (by slot), or nullptr = the stream's
 // current noise estimate (the first 160 floats of its noise-estimator state, LyraDecoder::RunComfortNoiseGenerator,
 // lyra/lyra_decoder.cc:328-340).  plan: nullptr = every slot runs; otherwise only slots with bit 2.
@@ -135,32 +110,10 @@ ComfortNoiseKernel(const uint8_t* __restrict__ blob, CngParams P, const int* __r
     else { xr0[FftIdx(i)] = vr; xi0[FftIdx(i)] = vi; xr0[FftIdx(N - i)] = vr; xi0[FftIdx(N - i)] = -vi; }
   }
   __syncthreads();
-  {                                                                            // stages 2, 4, 8 (bit reversal folded into the gather)
-    double xr[8], xi[8];
-    const int b7 = (int)(__brev((unsigned)tid) >> 25);
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const int j3 = ((j & 1) << 2) | (j & 2) | ((j & 4) >> 2);
-      const int i = b7 + 128 * j3;
-      xr[j] = xr0[FftIdx(i)];
-      xi[j] = xi0[FftIdx(i)];
-    }
-    IfftButterflies3<1>(xr, xi, 0, tw);
-#pragma unroll
-    for (int j = 0; j < 8; ++j) { re[FftIdx(8 * tid + j)] = xr[j]; im[FftIdx(8 * tid + j)] = xi[j]; }
-  }
-  __syncthreads();
-  IfftStages3<8>(re, im, 64 * (tid / 8) + tid % 8, tid % 8, tw);               // stages 16, 32, 64
-  __syncthreads();
-  IfftStages3<64>(re, im, 512 * (tid / 64) + tid % 64, tid % 64, tw);          // stages 128, 256, 512
-  __syncthreads();
-#pragma unroll
-  for (int m = 0; m < 4; ++m) {                                                // stage 1024
-    const int a = tid + NT * m, ia = FftIdx(a), ib = FftIdx(a + 512);
-    const double2 w = tw[511 + a];
-    FftButterfly(re[ia], im[ia], re[ib], im[ib], w.x, -w.y);
-  }
-  __syncthreads();
+  Fft1024<true>(re, im, tw, [&](int i, double& xr, double& xi) {
+    xr = xr0[FftIdx(i)];
+    xi = xi0[FftIdx(i)];
+  });
   // 1/N, synthesis window, overlap-add; emit one hop (ClipToInt16: clamp, truncate); shift the buffer by one hop
   double* wk = work + (size_t)stream * N;
   for (int i = tid; i < N; i += NT) {

@@ -1,6 +1,5 @@
 #!/bin/bash
 # usage: build_variant.sh name [-DFLAG ...]   -> devtools_build/liblyra_b200_<name>.so
-#   build_variant.sh phase -DLYRA_PHASE_PROF  -> the phase-stamp library of tools/phase_probe.py
 set -e
 cd "$(dirname "$0")/.."
 name=$1; shift
