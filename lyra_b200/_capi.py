@@ -112,7 +112,7 @@ def load():
     """Bind the product library (nvcc build). Fails loudly if it is missing."""
     global _product
     if _product is None:
-        _product = CApi(os.environ.get("LYRA_B200_LIB", PRODUCT_SO))   # the override is for kernel-variant experiments (tools/)
+        _product = CApi(PRODUCT_SO)
     return _product
 
 

@@ -1,14 +1,19 @@
 """GPU tier (H100) of per-stream sample rates (lyra_b200_set_stream_sample_rates): full-size dense device calls with their
 sub-batches engaged, both decoder modes, the asynchrony of the setter and bench.py's device schedule with mixed rates; against
 single-rate twin contexts and the oracle composition of tests/rate_cases.py."""
+import os
+import sys
+
 import numpy as np
 import pytest
 
 import mixed_rate_cases as mc
 import rate_cases as rc
-from conftest import read_wav_any
+from conftest import ROOT, read_wav_any
 from lyra_b200 import _capi
 from test_gpu_parity import TorchMem
+
+sys.path.insert(0, os.path.join(ROOT, "tools"))        # duplex_schedule
 
 pytestmark = pytest.mark.gpu
 
@@ -96,47 +101,17 @@ def test_bench_device_schedule_with_mixed_rates(gpu_api, mode, split):
     8 / 16 / 32 / 48 kHz interleaved, caller streams at priorities -1 / 0, encoder -> decoder events, 12 hops over 8 rotating
     slots queued with no host synchronisation.  Every hop's packets and PCM equal host-buffer calls on single-rate twin pairs."""
     import torch
-    rate, G, m, NBUF, hops, bits = 48000, 2, 1540, 8, 12, 64
-    H, P = rc.hop_of(rate), _capi.packet_bytes(bits)
+    import duplex_schedule as ds
+    rate, G, m, NBUF, hops, bits = 48000, 2, 1540, ds.NBUF, 12, 64
     n = G * m
     srate = mc.interleaved(m, mc.ALL_RATES)
     rng = np.random.default_rng(29)
-    host_pcm = [rng.integers(-8192, 8192, size=(n, H), dtype=np.int16) for _ in range(NBUF)]
-    d_pcm = [torch.from_numpy(x).cuda() for x in host_pcm]
-    d_pks = [torch.zeros((n, P), dtype=torch.uint8, device="cuda") for _ in range(NBUF)]
-    d_out = [torch.full((n, H), 0x5A5A, dtype=torch.int16, device="cuda") for _ in range(hops)]
-    pk_of_hop = [torch.zeros((n, P), dtype=torch.uint8, device="cuda") for _ in range(hops)]
-    groups = []
-    for g in range(G):
-        e_, d_ = _capi.Context(m, roles="encoder"), _capi.Context(m, roles="decoder")
-        d_.set_decoder_mode(mode)
-        gx, gy = torch.cuda.Stream(priority=-1), torch.cuda.Stream(priority=0)
-        for c, prio, st in ((e_, -1, gx), (d_, 0, gy)):
-            c.set_sample_rate(rate)
-            c.set_priority(prio)
-            c.set_stream(st.cuda_stream)
-            c.set_split(split)
-            c.set_stream_sample_rates(srate)
-        groups.append((e_, d_, gx, gy))
-    ev_pk = [[torch.cuda.Event() for _ in range(NBUF)] for _ in range(G)]
-    ev_free = [[torch.cuda.Event() for _ in range(NBUF)] for _ in range(G)]
+    host_pcm = [rng.integers(-8192, 8192, size=(n, rc.hop_of(rate)), dtype=np.int16) for _ in range(NBUF)]
+    sched = ds.Schedule(host_pcm, G, split, mode, bits, rate=rate, stream_rates=srate, keep_hops=hops)
+    ds.run([sched], hops)
     torch.cuda.synchronize()
-    for i in range(hops):
-        b = i % NBUF
-        for g, (e_, d_, gx, gy) in enumerate(groups):
-            off = g * m
-            if i >= NBUF:
-                gx.wait_event(ev_free[g][b])
-            e_.encode_device(m, d_pcm[b].data_ptr() + off * 2 * H, bits, d_pks[b].data_ptr() + off * P)
-            ev_pk[g][b].record(gx)
-            gy.wait_event(ev_pk[g][b])
-            d_.decode_device(m, d_pks[b].data_ptr() + off * P, 0, bits, d_out[i].data_ptr() + off * 2 * H)
-            with torch.cuda.stream(gy):
-                pk_of_hop[i][off:off + m].copy_(d_pks[b][off:off + m])
-            ev_free[g][b].record(gy)
-    torch.cuda.synchronize()
-    outs = [x.cpu().numpy() for x in d_out]
-    pks = [x.cpu().numpy() for x in pk_of_hop]
+    outs = [x.cpu().numpy() for x in sched.out]
+    pks = [x.cpu().numpy() for x in sched.kept_pks]
     sel = {r: np.nonzero(srate == r)[0] for r in mc.ALL_RATES}
     refs = []
     for _ in range(G):
@@ -161,5 +136,6 @@ def test_bench_device_schedule_with_mixed_rates(gpu_api, mode, split):
                 bad = np.nonzero((got[:, :rc.hop_of(r)] != want).any(axis=1))[0]
                 assert bad.size == 0, "PCM of hop %d group %d at %d Hz differs at streams %s" % (i, g, r, rows[bad[:8]])
                 assert not got[:, rc.hop_of(r):].any(), "row tails of hop %d group %d at %d Hz are not 0" % (i, g, r)
-    for c in [c for grp in groups for c in grp[:2]] + [c for pair in refs for p in pair.values() for c in p]:
+    sched.close()
+    for c in [c for pair in refs for p in pair.values() for c in p]:
         c.close()

@@ -2,13 +2,16 @@
 same seeded inputs; plus size-independent properties at BASELINE.json's full sizes."""
 import json
 import os
+import sys
 
 import numpy as np
 import pytest
 
 import parity_cases as pc
-from conftest import GOLDEN_DIR
+from conftest import GOLDEN_DIR, ROOT
 from lyra_b200 import _capi
+
+sys.path.insert(0, os.path.join(ROOT, "tools"))        # duplex_schedule
 
 pytestmark = pytest.mark.gpu
 
@@ -488,23 +491,19 @@ def _torch():
 @pytest.mark.parametrize("workload,mode,split", [("codec", "exact", 2), ("codec", "tensor", 3),
                                                  ("decode_plc", "exact", 3), ("decode_plc", "tensor", 2)])
 def test_bench_device_schedule(gpu_api, oracle, workload, mode, split):
-    """bench.py's device-resident pass (measure -> run_device) at a size where its sub-batches engage: G = 2 context pairs over
-    slices of shared buffers, caller streams at priorities -1 / 0, encoder -> decoder events, 12 hops over 8 rotating slots queued
-    with no host synchronisation.  2 x 1540 streams: 193 tiles per context, the last one partial, so a slice's last tile ends in
-    the middle of the shared buffer.  Every hop's output goes to its own buffer; all streams are compared with host-buffer calls
-    on a reference context per group, the streams at the slice edges with the oracle."""
-    torch = _torch()
+    """bench.py's device-resident pass (measure -> run_device, as tools/duplex_schedule.py runs it) at a size where its
+    sub-batches engage: G = 2 context pairs over slices of shared buffers, caller streams at priorities -1 / 0, encoder ->
+    decoder events, 12 hops over 8 rotating slots queued with no host synchronisation.  2 x 1540 streams: 193 tiles per context,
+    the last one partial, so a slice's last tile ends in the middle of the shared buffer.  Every hop's output goes to its own
+    buffer; all streams are compared with host-buffer calls on a reference context per group, the streams at the slice edges
+    with the oracle."""
+    import duplex_schedule as ds
     plc = workload == "decode_plc"
-    G, m, NBUF, hops, bits = 2, 1540, 8, 12, 64
-    n, P = G * m, _capi.packet_bytes(bits)
+    G, m, NBUF, hops, bits = 2, 1540, ds.NBUF, 12, 64
+    n = G * m
     tol = pc.TENSOR_PCM_TOL_LSB if mode == "tensor" else 0
     rng = np.random.default_rng(17)
     host_pcm = [pc.synth_pcm(rng, n, "noise" if b % 4 else "loud") for b in range(NBUF)]
-    d_pcm = [torch.from_numpy(x).cuda() for x in host_pcm]
-    d_pks = [torch.zeros((n, P), dtype=torch.uint8, device="cuda") for _ in range(NBUF)]
-    d_out = [torch.full((n, 320), 0x5A5A, dtype=torch.int16, device="cuda") for _ in range(hops)]
-    d_flags = [torch.full((n,), 0xAA, dtype=torch.uint8, device="cuda") for _ in range(hops)]
-    pk_of_hop = [torch.zeros((n, P), dtype=torch.uint8, device="cuda") for _ in range(hops)]
     edges = [0, m - 1, m, n - 1]
     if plc:
         # the workload's packets come from an encoder over the 8 input slots; bursts of 7 lost hops (slots 1..7) reach comfort
@@ -512,51 +511,18 @@ def test_bench_device_schedule(gpu_api, oracle, workload, mode, split):
         tmp = _capi.Context(n, roles="encoder")
         h_pks = [tmp.encode(x, bits) for x in host_pcm]
         tmp.close()
-        for b in range(NBUF):
-            d_pks[b].copy_(torch.from_numpy(h_pks[b]))
         burst = np.zeros(n, bool)
         burst[::5] = True
         burst[edges] = True
         h_masks = [((rng.random(n) >= 0.15) & ~(burst & (b > 0))).astype(np.uint8) for b in range(NBUF)]
-        d_masks = [torch.from_numpy(x).cuda() for x in h_masks]
-    groups = []
-    for g in range(G):
-        e_ = None if plc else _capi.Context(m, roles="encoder")
-        d_ = _capi.Context(m, roles="decoder")
-        d_.set_decoder_mode(mode)
-        gx, gy = torch.cuda.Stream(priority=-1), torch.cuda.Stream(priority=0)
-        d_.set_priority(0)
-        d_.set_stream(gy.cuda_stream)
-        d_.set_split(split)
-        if e_:
-            e_.set_priority(-1)
-            e_.set_stream(gx.cuda_stream)
-            e_.set_split(split)
-        groups.append((e_, d_, gx, gy))
-    ev_pk = [[torch.cuda.Event() for _ in range(NBUF)] for _ in range(G)]
-    ev_free = [[torch.cuda.Event() for _ in range(NBUF)] for _ in range(G)]
-    torch.cuda.synchronize()
-    for i in range(hops):
-        b = i % NBUF
-        for g, (e_, d_, gx, gy) in enumerate(groups):
-            off = g * m
-            if plc:
-                d_.decode_plc_device(m, d_pks[b].data_ptr() + off * P, d_masks[b].data_ptr() + off, bits,
-                                     d_out[i].data_ptr() + off * 640, d_flags[i].data_ptr() + off)
-                continue
-            if i >= NBUF:
-                gx.wait_event(ev_free[g][b])                   # the ring slot's previous packets have been decoded
-            e_.encode_device(m, d_pcm[b].data_ptr() + off * 640, bits, d_pks[b].data_ptr() + off * P)
-            ev_pk[g][b].record(gx)
-            gy.wait_event(ev_pk[g][b])
-            d_.decode_device(m, d_pks[b].data_ptr() + off * P, 0, bits, d_out[i].data_ptr() + off * 640)
-            with torch.cuda.stream(gy):                        # keep this hop's packets before the slot is reused
-                pk_of_hop[i][off:off + m].copy_(d_pks[b][off:off + m])
-            ev_free[g][b].record(gy)
-    torch.cuda.synchronize()
-    outs = [x.cpu().numpy() for x in d_out]
-    flags = [x.cpu().numpy() for x in d_flags]
-    pks = [x.cpu().numpy() for x in pk_of_hop]
+        sched = ds.Schedule(h_pks, G, split, mode, bits, masks=h_masks, keep_hops=hops)
+    else:
+        sched = ds.Schedule(host_pcm, G, split, mode, bits, keep_hops=hops)
+    ds.run([sched], hops)
+    _torch().cuda.synchronize()
+    outs = [x.cpu().numpy() for x in sched.out]
+    flags = [x.cpu().numpy() for x in sched.flags] if plc else None
+    pks = None if plc else [x.cpu().numpy() for x in sched.kept_pks]
     # reference: one context per group (the comfort-noise seed of a stream is the context's seed plus its id in that context)
     refs = [(None if plc else _capi.Context(m, roles="encoder"), _capi.Context(m, roles="decoder")) for _ in range(G)]
     for _, rd in refs:
@@ -590,7 +556,8 @@ def test_bench_device_schedule(gpu_api, oracle, workload, mode, split):
             d = int(np.abs(outs[i][s].astype(int) - opcm.astype(int)).max())
             assert d <= tol, "hop %d stream %d: max |PCM - oracle| %d" % (i, s, d)
     assert not plc or seen_cn
-    for c in [c for grp in groups for c in grp[:2]] + [c for r in refs for c in r]:
+    sched.close()
+    for c in [c for r in refs for c in r]:
         if c is not None:
             c.close()
 

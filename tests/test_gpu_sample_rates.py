@@ -1,14 +1,19 @@
 """GPU tier (H100) of the fused codec calls at 8 / 32 / 48 kHz (lyra_b200_set_sample_rate): every rate, full-size dense calls with
 their sub-batches engaged, both decoder modes, caller CUDA streams; against the oracle composition of tests/rate_cases.py and
 against the host-buffer twins."""
+import os
+import sys
+
 import numpy as np
 import pytest
 
 import parity_cases as pc
 import rate_cases as rc
-from conftest import read_wav_any
+from conftest import ROOT, read_wav_any
 from lyra_b200 import _capi
 from test_gpu_parity import TorchMem
+
+sys.path.insert(0, os.path.join(ROOT, "tools"))        # duplex_schedule
 
 pytestmark = pytest.mark.gpu
 
@@ -68,47 +73,18 @@ def test_bench_device_schedule_at_48khz(gpu_api, oracle, mode, split):
     Every hop's output is kept; all streams are compared with host-buffer calls on one reference pair per group, the streams at
     the slice edges with the oracle composition."""
     import torch
-    rate, G, m, NBUF, hops, bits = 48000, 2, 1540, 8, 12, 64
-    hop = rc.hop_of(rate)
-    n, P = G * m, _capi.packet_bytes(bits)
+    import duplex_schedule as ds
+    rate, G, m, NBUF, hops, bits = 48000, 2, 1540, ds.NBUF, 12, 64
+    n = G * m
     tol = pc.TENSOR_PCM_TOL_LSB if mode == "tensor" else 0
     rng = np.random.default_rng(23)
-    host_pcm = [rng.integers(-8192, 8192, size=(n, hop), dtype=np.int16) for _ in range(NBUF)]
-    d_pcm = [torch.from_numpy(x).cuda() for x in host_pcm]
-    d_pks = [torch.zeros((n, P), dtype=torch.uint8, device="cuda") for _ in range(NBUF)]
-    d_out = [torch.full((n, hop), 0x5A5A, dtype=torch.int16, device="cuda") for _ in range(hops)]
-    pk_of_hop = [torch.zeros((n, P), dtype=torch.uint8, device="cuda") for _ in range(hops)]
+    host_pcm = [rng.integers(-8192, 8192, size=(n, rc.hop_of(rate)), dtype=np.int16) for _ in range(NBUF)]
     edges = [0, m - 1, m, n - 1]
-    groups = []
-    for g in range(G):
-        e_, d_ = _capi.Context(m, roles="encoder"), _capi.Context(m, roles="decoder")
-        d_.set_decoder_mode(mode)
-        gx, gy = torch.cuda.Stream(priority=-1), torch.cuda.Stream(priority=0)
-        for c, prio, st in ((e_, -1, gx), (d_, 0, gy)):
-            c.set_sample_rate(rate)
-            c.set_priority(prio)
-            c.set_stream(st.cuda_stream)
-            c.set_split(split)
-        groups.append((e_, d_, gx, gy))
-    ev_pk = [[torch.cuda.Event() for _ in range(NBUF)] for _ in range(G)]
-    ev_free = [[torch.cuda.Event() for _ in range(NBUF)] for _ in range(G)]
+    sched = ds.Schedule(host_pcm, G, split, mode, bits, rate=rate, keep_hops=hops)
+    ds.run([sched], hops)
     torch.cuda.synchronize()
-    for i in range(hops):
-        b = i % NBUF
-        for g, (e_, d_, gx, gy) in enumerate(groups):
-            off = g * m
-            if i >= NBUF:
-                gx.wait_event(ev_free[g][b])
-            e_.encode_device(m, d_pcm[b].data_ptr() + off * 2 * hop, bits, d_pks[b].data_ptr() + off * P)
-            ev_pk[g][b].record(gx)
-            gy.wait_event(ev_pk[g][b])
-            d_.decode_device(m, d_pks[b].data_ptr() + off * P, 0, bits, d_out[i].data_ptr() + off * 2 * hop)
-            with torch.cuda.stream(gy):
-                pk_of_hop[i][off:off + m].copy_(d_pks[b][off:off + m])
-            ev_free[g][b].record(gy)
-    torch.cuda.synchronize()
-    outs = [x.cpu().numpy() for x in d_out]
-    pks = [x.cpu().numpy() for x in pk_of_hop]
+    outs = [x.cpu().numpy() for x in sched.out]
+    pks = [x.cpu().numpy() for x in sched.kept_pks]
     refs = []
     for _ in range(G):
         re, rd = _capi.Context(m, roles="encoder"), _capi.Context(m, roles="decoder")
@@ -131,5 +107,6 @@ def test_bench_device_schedule_at_48khz(gpu_api, oracle, mode, split):
             assert bytes(pks[i][s]) == opkt, (i, s)
             d = int(np.abs(outs[i][s].astype(int) - oracles[s].decode(opkt, bits).astype(int)).max())
             assert d <= tol, "hop %d stream %d: max |PCM - oracle| %d" % (i, s, d)
-    for c in [c for grp in groups for c in grp[:2]] + [c for r in refs for c in r]:
+    sched.close()
+    for c in [c for r in refs for c in r]:
         c.close()

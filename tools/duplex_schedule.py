@@ -1,0 +1,111 @@
+"""bench.py's device-resident duplex schedule (measure -> run_device, the non-serial branch), written once for the GPU tests that
+tie it to the oracle and for tools/schedule_bench.py.
+
+Each group is an encoder-only and a decoder-only context of m streams, installed on CUDA streams of their own at priorities
+-1 / 0, over rows [g*m, (g+1)*m) of shared input, packet and output buffers.  Hop i uses slot i % 8: its encode waits until
+the slot's previous packets have been decoded, its decode waits for its packets through an event, and nothing synchronises
+the host.  The decode_plc workload runs decode_plc_device on the decoder contexts alone, over caller-supplied packets and
+received masks.
+"""
+import numpy as np
+import torch
+
+from lyra_b200 import _capi
+
+NBUF = 8
+
+
+def _row(t, g, m):
+    """Device address of row g * m of a contiguous tensor."""
+    return t.data_ptr() + g * m * t.stride(0) * t.element_size()
+
+
+class Schedule:
+    def __init__(self, slots, groups, split, mode, bits=64, rate=16000, stream_rates=None, masks=None, keep_hops=0):
+        """slots: NBUF host arrays of n rows, the input PCM (rate // 50 samples per row), or with `masks` (the decode_plc
+        workload) the packets; masks: NBUF received masks of n entries.  stream_rates: the per-stream rates of every group's
+        m streams.  keep_hops: hop i < keep_hops writes its own output (and flag) buffer and keeps a copy of its packets, and
+        the schedule runs at most keep_hops hops; with 0 every hop writes one shared output."""
+        n = len(slots[0])
+        self.n, self.m, self.bits, self.keep_hops = n, n // groups, bits, keep_hops
+        self.plc = masks is not None
+        dev = lambda a: torch.from_numpy(np.ascontiguousarray(a)).cuda()   # noqa: E731
+        if self.plc:
+            self.pks, self.masks = [dev(x) for x in slots], [dev(x) for x in masks]
+        else:
+            self.pcm = [dev(x) for x in slots]
+            self.pks = [torch.zeros((n, _capi.packet_bytes(bits)), dtype=torch.uint8, device="cuda") for _ in range(NBUF)]
+            self.kept_pks = [torch.zeros_like(self.pks[0]) for _ in range(keep_hops)]
+        outs = max(keep_hops, 1)
+        self.out = [torch.full((n, rate // 50), 0x5A5A, dtype=torch.int16, device="cuda") for _ in range(outs)]
+        self.flags = [torch.full((n,), 0xAA, dtype=torch.uint8, device="cuda") for _ in range(outs)] if self.plc else None
+        self.groups = []
+        for _ in range(groups):
+            e_ = None if self.plc else _capi.Context(self.m, roles="encoder")
+            d_ = _capi.Context(self.m, roles="decoder")
+            gx, gy = torch.cuda.Stream(priority=-1), torch.cuda.Stream(priority=0)
+            for c, prio, st in ((e_, -1, gx), (d_, 0, gy)):
+                if c is None:
+                    continue
+                if rate != 16000:
+                    c.set_sample_rate(rate)
+                c.set_priority(prio)
+                c.set_stream(st.cuda_stream)
+                c.set_split(split)
+                if stream_rates is not None:
+                    c.set_stream_sample_rates(stream_rates)
+            d_.set_decoder_mode(mode)
+            self.groups.append((e_, d_, gx, gy))
+        self.ev_pk = [[torch.cuda.Event() for _ in range(NBUF)] for _ in range(groups)]      # [group][slot] packets written
+        self.ev_free = [[torch.cuda.Event() for _ in range(NBUF)] for _ in range(groups)]    # ... and consumed
+        torch.cuda.synchronize()          # the buffers above were filled on the current stream, the settings on the groups'
+
+    def hop(self, i):
+        """Hop i of every group."""
+        b, o, m, bits = i % NBUF, i if self.keep_hops else 0, self.m, self.bits
+        for g, (e_, d_, gx, gy) in enumerate(self.groups):
+            pk, out = _row(self.pks[b], g, m), _row(self.out[o], g, m)
+            if self.plc:
+                d_.decode_plc_device(m, pk, _row(self.masks[b], g, m), bits, out, _row(self.flags[o], g, m))
+                continue
+            if i >= NBUF:
+                gx.wait_event(self.ev_free[g][b])
+            e_.encode_device(m, _row(self.pcm[b], g, m), bits, pk)
+            self.ev_pk[g][b].record(gx)
+            gy.wait_event(self.ev_pk[g][b])
+            d_.decode_device(m, pk, 0, bits, out)
+            if self.keep_hops:
+                with torch.cuda.stream(gy):                # before the slot is reused
+                    self.kept_pks[i][g * m:(g + 1) * m].copy_(self.pks[b][g * m:(g + 1) * m])
+            self.ev_free[g][b].record(gy)
+
+    def close(self):
+        for e_, d_, _, _ in self.groups:
+            for c in (e_, d_):
+                if c is not None:
+                    c.close()
+
+
+def run(schedules, hops):
+    """Hops 0 .. hops-1, the schedules interleaved hop by hop."""
+    for i in range(hops):
+        for s in schedules:
+            s.hop(i)
+
+
+def timed(schedules, hops):
+    """Frames/s of run(schedules, hops), timed with CUDA events on a timer stream that every work stream forks from and joins
+    into: nothing of the run starts before the first event, and the second waits for all of it."""
+    timer = torch.cuda.Stream()
+    work = [st for s in schedules for grp in s.groups for st in grp[2:]]
+    torch.cuda.synchronize()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record(timer)
+    for st in work:
+        st.wait_stream(timer)
+    run(schedules, hops)
+    for st in work:
+        timer.wait_stream(st)
+    e1.record(timer)
+    torch.cuda.synchronize()
+    return sum(s.n for s in schedules) * hops / (e0.elapsed_time(e1) / 1e3)

@@ -11,12 +11,10 @@ from lyra_b200 import _capi  # noqa
 
 def main():
     n = int(sys.argv[1]) if len(sys.argv) > 1 else 4096
-    so = sys.argv[2] if len(sys.argv) > 2 else os.path.join(ROOT, "lyra_b200", "liblyra_b200.so")
-    api = _capi.CApi(so)
     rng = np.random.default_rng(0)
     pcm = rng.integers(-8192, 8192, size=(n, 320), dtype=np.int16)
     for mode in ("exact", "tensor"):
-        ctx = _capi.Context(n, capi=api)
+        ctx = _capi.Context(n)
         ctx.set_decoder_mode(mode)
         ctx.set_split(1)
         for _ in range(3):

@@ -1,0 +1,136 @@
+"""Throughput of bench.py's device-resident duplex schedule (tools/duplex_schedule.py) in named configurations, alternated run by
+run in one process so that clock and thermal drift hit them alike:
+  16k, 8k, 32k, 48k  every stream at that context rate (lyra_b200_set_sample_rate) in --groups context pairs; 16k is the
+                     benchmark's workload;
+  mixed              --groups pairs at row rate 48 kHz, the streams at 8 / 16 / 32 / 48 kHz interleaved
+                     (lyra_b200_set_stream_sample_rates) so that every tile mixes the four rates;
+  split              the same traffic split by rate: one context pair per rate with a quarter of the streams each (what a
+                     server without per-stream rates runs);
+  mixed-counters     16k with the odd lanes of every context set back to their state at creation (copy_streams from -1) after
+                     the warm-up, so odd and even lanes stay 10 hops apart and every tile takes the per-stream hop-counter path
+                     of the depthwise convolutions instead of the shared-counter fast path.
+Prints one line per run, then every configuration's median, spread and ratio to the first configuration, the card's name,
+power limit and median SM clock over the timed runs, and a JSON line.  --profile-hops adds a torch.profiler pass per
+configuration, separate from the timed runs: ResampleKernel's mean device time per launch.
+
+  python tools/schedule_bench.py [--configs 16k,48k,8k,mixed,split,mixed-counters] [--streams 4096] [--hops 200] [--runs 5]
+"""
+import argparse
+import json
+import os
+import subprocess
+import sys
+
+import numpy as np
+import torch
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+import bench  # noqa: E402
+import duplex_schedule as ds  # noqa: E402
+
+RATES = (8000, 16000, 32000, 48000)
+CONFIGS = ("16k", "8k", "32k", "48k", "mixed", "split", "mixed-counters")
+
+
+def power_limit():
+    try:
+        out = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i", "0"], capture_output=True,
+                             text=True, timeout=30)
+        return out.stdout.strip() or None
+    except Exception:
+        return None
+
+
+def make(name, args):
+    """The schedules of one configuration."""
+    def sched(n, groups, rate=16000, stream_rates=None):
+        rng = np.random.default_rng(1234)
+        pcm = [rng.integers(-8192, 8192, size=(n, rate // 50), dtype=np.int16) for _ in range(ds.NBUF)]
+        return ds.Schedule(pcm, groups, args.split, args.decoder_mode, args.bits, rate=rate, stream_rates=stream_rates)
+
+    n, g = args.streams, args.groups
+    if name == "mixed":
+        return [sched(n, g, 48000, np.array([RATES[k % len(RATES)] for k in range(n // g)], dtype=np.int32))]
+    if name == "split":
+        return [sched(n // len(RATES), 1, r) for r in RATES]
+    return [sched(n, g, 16000 if name == "mixed-counters" else int(name[:-1]) * 1000)]
+
+
+def resample_kernel_us(scheds, hops):
+    """Mean device time of one ResampleKernel launch (torch.profiler, CUDA activity) over `hops` hops, and the launch count."""
+    from torch.profiler import ProfilerActivity, profile
+    torch.cuda.synchronize()
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        ds.run(scheds, hops)
+        torch.cuda.synchronize()
+    times = [ev.time_range.elapsed_us() for ev in prof.events() if "ResampleKernel" in ev.name]
+    return (sum(times) / len(times) if times else None), len(times)
+
+
+def main():
+    ap = argparse.ArgumentParser(description=__doc__.split("\n\n")[0], formatter_class=argparse.RawDescriptionHelpFormatter)
+    ap.add_argument("--configs", default="16k,48k,8k,mixed,split,mixed-counters", help="comma-separated, from " + ",".join(CONFIGS))
+    ap.add_argument("--streams", type=int, default=4096)
+    ap.add_argument("--hops", type=int, default=200, help="hops per timed run")
+    ap.add_argument("--runs", type=int, default=5, help="runs per configuration, alternating the configurations")
+    ap.add_argument("--groups", type=int, default=2)
+    ap.add_argument("--split", type=int, default=2)
+    ap.add_argument("--bits", type=int, default=64, help="64 bits per 20 ms hop = 3.2 kbps")
+    ap.add_argument("--decoder-mode", default="tensor", choices=["exact", "tensor"])
+    ap.add_argument("--profile-hops", type=int, default=0, help="hops of the ResampleKernel profiler pass (0: none)")
+    args = ap.parse_args()
+    names = args.configs.split(",")
+    bad = [k for k in names if k not in CONFIGS]
+    if bad:
+        ap.error("unknown configuration %s" % ", ".join(bad))
+    if not torch.cuda.is_available():
+        raise SystemExit("schedule_bench needs a CUDA device")
+    configs = {k: make(k, args) for k in names}
+    for scheds in configs.values():
+        ds.run(scheds, ds.NBUF + 2)          # warm-up: first launches, stream maps; every stream at hop counter 10
+    torch.cuda.synchronize()
+    if "mixed-counters" in configs:
+        s = configs["mixed-counters"][0]
+        odd = np.arange(1, s.m, 2, dtype=np.int32)
+        for e_, d_, _, _ in s.groups:
+            for c in (e_, d_):
+                c.copy_streams(np.full(odd.size, -1, np.int32), odd)   # odd lanes back to hop counter 0
+        torch.cuda.synchronize()
+    fps = {k: [] for k in names}
+    sampler = bench.ClockSampler(0, "GPU-%s" % torch.cuda.get_device_properties(0).uuid)
+    sampler.start()
+    for run in range(args.runs):
+        for k, scheds in configs.items():
+            v = ds.timed(scheds, args.hops)
+            fps[k].append(v)
+            print("run %d  %-14s  %.3f M frames/s" % (run, k, v / 1e6), flush=True)
+    clocks = sampler.stop()
+    kernel = {}
+    if args.profile_hops:
+        for k, scheds in configs.items():
+            us, count = resample_kernel_us(scheds, args.profile_hops)
+            kernel[k] = {"us_per_launch": us, "launches": count}
+    for scheds in configs.values():
+        for s in scheds:
+            s.close()
+    base = names[0]
+    med = {k: float(np.median(v)) for k, v in fps.items()}
+    res = {
+        "gpu": torch.cuda.get_device_name(), "power_limit": power_limit(), "clocks": clocks, "streams": args.streams,
+        "bits": args.bits, "decoder_mode": args.decoder_mode, "split": args.split, "groups": args.groups, "hops_per_run": args.hops,
+        "frames_per_s": fps, "median_frames_per_s": med, "spread": {k: [min(v) / med[k], max(v) / med[k]] for k, v in fps.items()},
+        "ratio_to_" + base: {k: v / med[base] for k, v in med.items()}, "resample_kernel": kernel,
+    }
+    for k in names:
+        print("%-14s: median %.3f M frames/s (runs %.3f-%.3f), %.3f x %s" % (k, med[k] / 1e6, min(fps[k]) / 1e6, max(fps[k]) / 1e6,
+                                                                         med[k] / med[base], base))
+    for k, v in kernel.items():
+        if v["launches"]:
+            print("ResampleKernel in %s: %.1f us per launch (%d launches)" % (k, v["us_per_launch"], v["launches"]))
+    print("GPU %s, power limit %s, median SM clock %s MHz" % (res["gpu"], res["power_limit"], clocks["sm_mhz"]))
+    print(json.dumps(res))
+
+
+if __name__ == "__main__":
+    main()

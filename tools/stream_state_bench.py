@@ -1,14 +1,10 @@
-"""Cost of moving live streams (lyra_b200_copy_streams / _export_streams / _import_streams) and of what a move leaves behind.
+"""Cost of moving live streams (lyra_b200_copy_streams / _export_streams / _import_streams): copy_streams of 1, 64 and 1024
+streams inside a 4096-stream context (CUDA events around --reps calls on the installed stream), and export / import of 4096
+streams to / from page-locked host memory (host clock; both calls end in a device synchronise).  Algorithmic bytes = record
+payload x streams, read + write.  What a move leaves behind, tiles whose streams run on different hop counters, is the
+mixed-counters configuration of tools/schedule_bench.py.
 
-1. copy_streams of 1, 64 and 1024 streams inside a 4096-stream context (CUDA events around --reps calls on the installed
-   stream), and export / import of 4096 streams to / from page-locked host memory (host clock; both calls end in a device
-   synchronise).  Algorithmic bytes = record payload x streams, read + write.
-2. tools/rate_bench.py's device-resident duplex schedule at 4096 streams, 16 kHz: every stream on the same hop counter (the
-   shared-counter fast path of the depthwise convolutions) against every tile mixed (copy_streams of the state at creation
-   into every odd stream after the warm-up, so odd and even lanes stay 10 hops apart: every tile takes the per-stream path).
-   The two run alternately in one process; the medians are reported.
-
-  python tools/stream_state_bench.py [--streams 4096] [--runs 5] [--out DIR]
+  python tools/stream_state_bench.py [--streams 4096] [--out DIR]
 """
 import argparse
 import ctypes as C
@@ -23,7 +19,7 @@ import torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 from lyra_b200 import _capi  # noqa: E402
-from rate_bench import NBUF, Schedule, power_limit  # noqa: E402
+from schedule_bench import power_limit  # noqa: E402
 
 HBM_TBPS = 3.35          # H100 SXM data sheet
 
@@ -78,42 +74,11 @@ def export_import_times(n_streams, reps):
     return res, rb
 
 
-def mixed_counter_cost(n_streams, runs, hops, groups, split, bits, mode):
-    aligned = Schedule(16000, n_streams, groups, split, bits, mode)
-    mixed = Schedule(16000, n_streams, groups, split, bits, mode)
-    for s in (aligned, mixed):
-        s.run(NBUF + 2)                  # every stream at hop counter 10
-    torch.cuda.synchronize()
-    odd = np.arange(1, n_streams // groups, 2, dtype=np.int32)
-    for e_, d_, _, _ in mixed.groups:
-        for c in (e_, d_):
-            c.copy_streams(np.full(odd.size, -1, np.int32), odd)        # odd lanes back to counter 0
-    torch.cuda.synchronize()
-    fps = {"aligned": [], "mixed": []}
-    for r in range(runs):
-        for name, s in (("aligned", aligned), ("mixed", mixed)):
-            v = s.timed(hops)
-            fps[name].append(v)
-            print("run %d  %-7s  %.3f M frames/s" % (r, name, v / 1e6), flush=True)
-    med = {k: float(np.median(v)) for k, v in fps.items()}
-    for s in (aligned, mixed):
-        s.close()
-    print("duplex %d streams 16 kHz: aligned %.3f, every tile mixed %.3f M frames/s (%.3f x)" % (
-        n_streams, med["aligned"] / 1e6, med["mixed"] / 1e6, med["mixed"] / med["aligned"]), flush=True)
-    return {"frames_per_s": fps, "median_frames_per_s": med, "mixed_over_aligned": med["mixed"] / med["aligned"]}
-
-
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--streams", type=int, default=4096)
     ap.add_argument("--copy-sizes", default="1,64,1024")
     ap.add_argument("--reps", type=int, default=50)
-    ap.add_argument("--runs", type=int, default=5, help="alternating aligned / mixed runs of the duplex schedule")
-    ap.add_argument("--hops", type=int, default=200, help="hops per timed run")
-    ap.add_argument("--groups", type=int, default=2)
-    ap.add_argument("--split", type=int, default=2)
-    ap.add_argument("--bits", type=int, default=64)
-    ap.add_argument("--decoder-mode", default="tensor", choices=["exact", "tensor"])
     ap.add_argument("--out", default=None, help="directory for the JSON result")
     args = ap.parse_args()
     if not torch.cuda.is_available():
@@ -122,7 +87,6 @@ def main():
     print("GPU %s, power limit %s" % (res["gpu"], res["power_limit"]), flush=True)
     res["copy_streams"] = copy_times(args.streams, [int(x) for x in args.copy_sizes.split(",")], args.reps)
     res["export_import"], res["record_bytes"] = export_import_times(args.streams, 3)
-    res["duplex"] = mixed_counter_cost(args.streams, args.runs, args.hops, args.groups, args.split, args.bits, args.decoder_mode)
     line = json.dumps(res)
     if args.out:
         os.makedirs(args.out, exist_ok=True)
