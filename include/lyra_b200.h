@@ -132,6 +132,27 @@ int lyra_b200_set_stream_sample_rates(lyra_b200_ctx* ctx, const int32_t* stream_
 /* rates_hz[k] = the rate stream stream_ids[k] (NULL: k) runs at; an id may be listed more than once.  Ordered on the installed
  * stream behind the work queued there; returns when done. */
 int lyra_b200_stream_sample_rates(lyra_b200_ctx* ctx, const int32_t* stream_ids, int n, int32_t* rates_hz);
+/* Per-stream bit rates: the stream's own bit count in one role, i.e. the bit rate of its LyraEncoder (LyraEncoder::set_bitrate,
+ * lyra/lyra_encoder.cc:158-166) or of the packets its LyraDecoder receives (lyra/lyra_decoder.cc:172-184,
+ * lyra/lyra_config.h:99-115).  role is LYRA_B200_ROLE_ENCODER or LYRA_B200_ROLE_DECODER and must be a role of the context; the
+ * two words of a stream are independent.  bits[k] is 0 (follow the call's num_bits) or a bit count the calls accept: a multiple
+ * of 4 in 4..184.
+ *   In the fused calls and their *_device twins num_bits keeps its meaning for streams whose word is 0 and sets the packet row
+ *   stride, ceil(num_bits / 8).  A stream with its own count b: the encoders write its packet at b bits into the first
+ *   ceil(b / 8) bytes of its row and zeros over the rest; lyra_b200_encode_dtx reports packet_bytes 0 or ceil(b / 8); the
+ *   decoders read a received packet as b bits from the first ceil(b / 8) bytes of its row and ignore the rest.  Lost packets,
+ *   DTX and comfort noise behave as before.  A call returns LYRA_B200_EINVAL and queues nothing when a stream it lists has its
+ *   own count above the call's num_bits; streams it does not list do not constrain it.
+ *   quantize / dequantize ignore the words.
+ * Changing a word between hops is LyraEncoder::set_bitrate: the next packet comes out at the new size, and the networks,
+ * estimators and hop counters carry on.  A bad count, a role the context lacks (or not exactly one role), an id out of range or
+ * a repeated id returns LYRA_B200_EINVAL and changes nothing.  Asynchronous like lyra_b200_set_stream_sample_rates: queued on
+ * the installed stream, no host synchronisation.  lyra_b200_reset and copy_streams from -1 set both words to 0; copy, export and
+ * import carry them.  A context in which no stream has its own count launches exactly what it launches without this call. */
+int lyra_b200_set_stream_bits(lyra_b200_ctx* ctx, int role, const int32_t* stream_ids, int n, const int32_t* bits);
+/* bits[k] = the word of stream stream_ids[k] (NULL: k) in `role` (0: it follows the call); an id may be listed more than once.
+ * Ordered on the installed stream behind the work queued there; returns when done. */
+int lyra_b200_stream_bits(lyra_b200_ctx* ctx, int role, const int32_t* stream_ids, int n, int32_t* bits);
 
 /* LyraEncoder::Encode without DTX (lyra/lyra_encoder.cc:113-156) for n streams:
  * pcm[n][sample_rate / 50] -> packets[n][ceil(num_bits/8)] (pcm[n][320] at the default 16 kHz; lyra_b200_set_sample_rate).

@@ -80,6 +80,8 @@ class CApi:
             "lyra_b200_sample_rate": (ci, [vp]),
             "lyra_b200_set_stream_sample_rates": (ci, [vp, vp, ci, vp]),
             "lyra_b200_stream_sample_rates": (ci, [vp, vp, ci, vp]),
+            "lyra_b200_set_stream_bits": (ci, [vp, ci, vp, ci, vp]),
+            "lyra_b200_stream_bits": (ci, [vp, ci, vp, ci, vp]),
             "lyra_b200_stream_state_bytes": (ci, [vp]),
             "lyra_b200_export_streams": (ci, [vp, vp, ci, vp]),
             "lyra_b200_import_streams": (ci, [vp, vp, ci, vp]),
@@ -101,7 +103,8 @@ class CApi:
                "lyra_b200_profile_read", "lyra_b200_noise_estimate", "lyra_b200_decode_plc", "lyra_b200_decode_plc_device",
                "lyra_b200_plc_get_state", "lyra_b200_plc_set_state", "lyra_b200_cng_generate", "lyra_b200_set_cng_seed",
                "lyra_b200_encode_dtx", "lyra_b200_encode_dtx_device", "lyra_b200_resample", "lyra_b200_set_sample_rate",
-               "lyra_b200_sample_rate", "lyra_b200_set_stream_sample_rates", "lyra_b200_stream_sample_rates", "lyra_b200_stream_state_bytes", "lyra_b200_export_streams", "lyra_b200_import_streams",
+               "lyra_b200_sample_rate", "lyra_b200_set_stream_sample_rates", "lyra_b200_stream_sample_rates", "lyra_b200_set_stream_bits",
+               "lyra_b200_stream_bits", "lyra_b200_stream_state_bytes", "lyra_b200_export_streams", "lyra_b200_import_streams",
                "lyra_b200_copy_streams"]
 
 
@@ -233,6 +236,22 @@ class Context:
         n = ids.size if ids is not None else (self.max_streams if n is None else n)
         out = np.empty(n, dtype=np.int32)
         self._check(self.api.lib.lyra_b200_stream_sample_rates(self.h, _ptr(ids), n, _ptr(out)))
+        return out
+
+    def set_stream_bits(self, role, bits, stream_ids=None):
+        """Streams `stream_ids` (default: 0..len(bits)-1) of role "encoder" or "decoder" run the fused calls at bits[k] bits per
+        packet (a multiple of 4 in 4..184; 0: the call's num_bits, which also sets the packet row size).  Asynchronous on the
+        installed stream."""
+        b = np.ascontiguousarray(bits, dtype=np.int32).reshape(-1)
+        ids = _ids(stream_ids, b.size)
+        self._check(self.api.lib.lyra_b200_set_stream_bits(self.h, self.ROLES.get(role, role), _ptr(ids), b.size, _ptr(b)))
+
+    def stream_bits(self, role, stream_ids=None, n=None):
+        """The word of each listed stream in `role` (default: streams 0..n-1, n = max_streams) -> int32[n]; 0: the call's."""
+        ids = None if stream_ids is None else np.ascontiguousarray(stream_ids, dtype=np.int32).reshape(-1)
+        n = ids.size if ids is not None else (self.max_streams if n is None else n)
+        out = np.empty(n, dtype=np.int32)
+        self._check(self.api.lib.lyra_b200_stream_bits(self.h, self.ROLES.get(role, role), _ptr(ids), n, _ptr(out)))
         return out
 
     @property

@@ -47,7 +47,7 @@ struct lyra_b200_ctx {
   // (nullptr: zero), hop counter `n18` (nullptr: none; initially 0).  `reset` = false: lyra_b200_reset leaves the entry alone
   // (lyra_b200_resample's delay lines).  `kind` (StreamStateKind) marks the words a record does not carry verbatim; `check`
   // is what import validates in a record's payload besides the hop counter.
-  enum Check { kCheckNone, kCheckPlc, kCheckResamplerPos, kCheckStreamRate };
+  enum Check { kCheckNone, kCheckPlc, kCheckResamplerPos, kCheckStreamRate, kCheckStreamBits };
   struct StateEntry {
     StreamStateEntry e;              // e.offset is set by BuildStateTable
     bool reset;
@@ -104,6 +104,14 @@ struct lyra_b200_ctx {
   bool rate_override = false;                    // some stream may run at another rate than sample_rate
   ByRate<NoiseParams> enc_noise_params{};        // the encoder-side estimators' constants and extractor tables, by stream rate
   ByRate<LogMelParams> enc_logmel{};
+  // lyra_b200_set_stream_bits: one word per stream and role ([0] encoder, [1] decoder; nullptr when the context lacks the role),
+  // 0 = the call's num_bits, otherwise the stream's own bit count.  Every change starts on the host (the setter, copy_streams,
+  // import_streams, reset), so bits_mirror is an exact host image of the words in program order, which is also stream order: the
+  // calls check their num_bits against it without reading the device.  own_bits[r] counts the streams whose word is not 0; while
+  // it is 0 the RVQ kernels get no word pointer and the calls launch exactly what they launch without the feature.
+  int* d_stream_bits[2] = {nullptr, nullptr};
+  std::vector<int> bits_mirror[2];
+  int own_bits[2] = {0, 0};
   // device staging for the host-buffer API
   int16_t* d_pcm = nullptr;
   uint8_t* d_packets = nullptr;
@@ -141,14 +149,15 @@ struct lyra_b200_ctx {
   uint64_t launches = 0;
   // lyra_b200_set_graphs: the dense host-buffer encode / decode calls replay a captured CUDA graph (copies in, kernels of every
   // sub-batch, copies out) instead of re-issuing ~20 stream operations per call; one graph per (call shape, host buffers)
-  // (rates: rate_override, which adds the converters' launches at 16 kHz)
+  // (rates: rate_override, which adds the converters' launches at 16 kHz; bits: own_bits of the call's role, which hands the RVQ
+  // kernels the bits words)
   struct GraphKey {
     int kind, n, num_bits, mode, nsplit;
     const void *a, *b, *c;
-    bool rates;
+    bool rates, bits;
     bool operator==(const GraphKey& o) const {
       return kind == o.kind && n == o.n && num_bits == o.num_bits && mode == o.mode && nsplit == o.nsplit && a == o.a && b == o.b && c == o.c &&
-             rates == o.rates;
+             rates == o.rates && bits == o.bits;
     }
   };
   struct GraphEntry { GraphKey key; void* exec; uint64_t launches; };
@@ -265,6 +274,21 @@ bool BitsOk(lyra_b200_ctx* ctx, int num_bits) {
   return true;
 }
 
+// a bit count lyra_b200_set_stream_bits and import accept for a stream's own word: one the calls accept
+bool StreamBitsOk(const lyra_b200_ctx* ctx, int bits) {
+  return bits > 0 && bits <= LYRA_B200_MAX_BITS && bits % ctx->spec.bits_per_stage == 0;
+}
+
+// the bits words of role index r (0 encoder, 1 decoder) as the RVQ kernels get them: nullptr while no stream has its own count
+const int* BitsWord(const lyra_b200_ctx* ctx, int r) { return ctx->own_bits[r] ? ctx->d_stream_bits[r] : nullptr; }
+
+// stream `id`'s word of role index r in the host mirror (and own_bits)
+void SetMirrorBits(lyra_b200_ctx* ctx, int r, int id, int bits) {
+  int& w = ctx->bits_mirror[r][(size_t)id];
+  ctx->own_bits[r] += (bits != 0) - (w != 0);
+  w = bits;
+}
+
 // A fresh stamp for ctx->id_seen: no stream is marked with it yet
 uint32_t NextIdGen(lyra_b200_ctx* ctx) {
   if (++ctx->id_gen == 0) { std::fill(ctx->id_seen.begin(), ctx->id_seen.end(), 0u); ctx->id_gen = 1; }
@@ -347,21 +371,23 @@ int LaunchEncoderNets(lyra_b200_ctx* ctx, const Part& p, const uint8_t* skip, co
                           ctx->d_blob, ctx->spec.enc, io, ctx->d_mid_enc, reinterpret_cast<float*>(ctx->d_state[1]), ctx->d_n18[1], d_features);
 }
 
+// bits_word (nullptr: every row at num_bits) and d_ids: the per-stream bit counts of the call's streams (RvqEncodeKernel)
 int LaunchQuantize(lyra_b200_ctx* ctx, const Part& p, const float* d_features, int num_bits, uint8_t* d_packets, int* d_indices,
-                   const uint8_t* d_skip = nullptr) {
+                   const uint8_t* d_skip = nullptr, const int* bits_word = nullptr, const int* d_ids = nullptr) {
   const int nq = num_bits / ctx->spec.bits_per_stage, pb = PacketBytes(num_bits);
   const int blocks = (p.nslots + kRvqSlotsPerBlock - 1) / kRvqSlotsPerBlock;
   return LAUNCH(2, RvqEncodeKernel, dim3((unsigned)blocks), dim3(kRvqThreads), (size_t)(2 * 1024 * 4 + kRvqSlotsPerBlock * (64 * 4 + 48 * 4)), p.st,
                 ctx->d_blob, ctx->spec.rvq, d_features + (size_t)p.slot0 * 64, p.nslots, nq, d_packets + (size_t)p.slot0 * pb, pb,
-                d_indices ? d_indices + (size_t)p.slot0 * 46 : nullptr, d_skip ? d_skip + p.slot0 : nullptr);
+                d_indices ? d_indices + (size_t)p.slot0 * 46 : nullptr, d_skip ? d_skip + p.slot0 : nullptr, bits_word, d_ids, p.slot0);
 }
 
-int LaunchDequantize(lyra_b200_ctx* ctx, const Part& p, const uint8_t* d_packets, const uint8_t* d_received, int num_bits, float* d_features) {
+int LaunchDequantize(lyra_b200_ctx* ctx, const Part& p, const uint8_t* d_packets, const uint8_t* d_received, int num_bits, float* d_features,
+                     const int* bits_word = nullptr, const int* d_ids = nullptr) {
   const int nq = num_bits / ctx->spec.bits_per_stage, pb = PacketBytes(num_bits);
   const int blocks = (p.nslots * 64 + 255) / 256;
   return LAUNCH(3, RvqDecodeKernel, dim3((unsigned)blocks), dim3(256), (size_t)0, p.st,
                 ctx->d_blob, ctx->spec.rvq, d_packets + (size_t)p.slot0 * pb, pb, d_received ? d_received + p.slot0 : nullptr, p.nslots, nq,
-                d_features + (size_t)p.slot0 * 64);
+                d_features + (size_t)p.slot0 * 64, bits_word, d_ids, p.slot0);
 }
 
 // Exact mode: DecoderKernelC<false> + DecoderKernelD, fp32 FMA chains bit-exact with the oracle.  Tensor mode: DecoderKernelC<true>
@@ -537,7 +563,7 @@ int RunEncode(lyra_b200_ctx* ctx, const CodecCall& c) {
       if (h.flags) CU(cudaMemcpyAsync(h.flags + p.slot0, d.flags + p.slot0, (size_t)p.nslots, cudaMemcpyDeviceToHost, p.st));
     }
     if ((rc = LaunchEncoderNets(ctx, p, skip, pcm16, ctx->d_features))) return rc;
-    if ((rc = LaunchQuantize(ctx, p, ctx->d_features, c.num_bits, d.packets_out, nullptr, skip))) return rc;
+    if ((rc = LaunchQuantize(ctx, p, ctx->d_features, c.num_bits, d.packets_out, nullptr, skip, BitsWord(ctx, 0), c.d_ids))) return rc;
     if (h.packets_out)
       CU(cudaMemcpyAsync(h.packets_out + (size_t)p.slot0 * pb, d.packets_out + (size_t)p.slot0 * pb, pb * (size_t)p.nslots, cudaMemcpyDeviceToHost, p.st));
     return LYRA_B200_OK;
@@ -561,7 +587,7 @@ int RunDecode(lyra_b200_ctx* ctx, const CodecCall& c) {
       CU(cudaMemcpyAsync(ctx->d_packets + (size_t)p.slot0 * pb, h.packets_in + (size_t)p.slot0 * pb, pb * (size_t)p.nslots, cudaMemcpyHostToDevice, p.st));
     if (h.received)
       CU(cudaMemcpyAsync(ctx->d_received + p.slot0, h.received + p.slot0, (size_t)p.nslots, cudaMemcpyHostToDevice, p.st));
-    if ((rc = LaunchDequantize(ctx, p, d.packets_in, d.received, c.num_bits, ctx->d_features))) return rc;
+    if ((rc = LaunchDequantize(ctx, p, d.packets_in, d.received, c.num_bits, ctx->d_features, BitsWord(ctx, 1), c.d_ids))) return rc;
     if ((rc = LaunchDecoderNets(ctx, p, nullptr, ctx->d_features, pcm16))) return rc;
     if (c.kind == kDecodeTrackNoise) {
       if ((rc = LaunchNoiseUpdate(ctx, p.st, c.d_ids, p.slot0, p.nslots, c.n, pcm16, d.received, d.flags, nullptr))) return rc;
@@ -594,7 +620,7 @@ int RunDecodePlc(lyra_b200_ctx* ctx, const CodecCall& c) {
     int rc = LYRA_B200_OK;
     if (h.packets_in)
       CU(cudaMemcpyAsync(ctx->d_packets + (size_t)p.slot0 * pb, h.packets_in + (size_t)p.slot0 * pb, pb * (size_t)p.nslots, cudaMemcpyHostToDevice, p.st));
-    if ((rc = LaunchDequantize(ctx, p, d.packets_in, d.received, c.num_bits, ctx->d_features))) return rc;
+    if ((rc = LaunchDequantize(ctx, p, d.packets_in, d.received, c.num_bits, ctx->d_features, BitsWord(ctx, 1), c.d_ids))) return rc;
     if ((rc = LaunchDecoderNets(ctx, p, ctx->d_skip, ctx->d_features, ctx->d_model_pcm))) return rc;
     if ((rc = LaunchComfortNoise(ctx, p.st, c.d_ids, p.slot0, p.nslots, c.n, nullptr, ctx->d_plan))) return rc;
     if ((rc = LAUNCH(kNoProf, PlcMixKernel, dim3((unsigned)p.nslots), dim3(320), (size_t)0, p.st,
@@ -762,8 +788,9 @@ int RunMaybeGraphed(lyra_b200_ctx* ctx, const lyra_b200_ctx::GraphKey& key, bool
 #endif
 }
 
-// Every fused codec call past its own pointer checks: role, bit count, tile map; the stream ids go to the device when the call's
-// chain has a kernel indexed by stream id (the converters, the noise estimators, the PLC kernels).  A host-buffer call runs on the
+// Every fused codec call past its own pointer checks: role, bit count (also against the listed streams' own counts, from the host
+// mirror), tile map; the stream ids go to the device when the call's chain has a kernel indexed by stream id (the converters, the
+// noise estimators, the PLC kernels, the RVQ kernels while some stream of the role has its own bit count).  A host-buffer call runs on the
 // context's staging buffers, a call without a flag buffer on the context's, and only the dense host-buffer encode / decode may
 // replay a graph.  A host-buffer call returns when its results are in the caller's buffers; a *_device twin never waits.
 int RunCodecCall(lyra_b200_ctx* ctx, CodecCall c) {
@@ -771,7 +798,16 @@ int RunCodecCall(lyra_b200_ctx* ctx, CodecCall c) {
   const int role = encoder ? LYRA_B200_ROLE_ENCODER : LYRA_B200_ROLE_DECODER;
   ENTER(role);
   if (!BitsOk(ctx, c.num_bits)) return LYRA_B200_EINVAL;
-  const bool by_id = Converts(ctx) || (c.kind != kEncode && c.kind != kDecode);
+  const int r = encoder ? 0 : 1;
+  const std::vector<int>& own = ctx->bits_mirror[r];
+  for (int k = 0; k < c.n && ctx->own_bits[r]; ++k) {
+    const int id = c.ids ? c.ids[k] : k;            // an id out of range is refused by PrepareMap
+    if (id >= 0 && id < ctx->max_streams && own[(size_t)id] > c.num_bits) {
+      ctx->err = "a listed stream's own bit count (lyra_b200_set_stream_bits) is above the call's num_bits";
+      return LYRA_B200_EINVAL;
+    }
+  }
+  const bool by_id = Converts(ctx) || (c.kind != kEncode && c.kind != kDecode) || ctx->own_bits[r];
   int rc = PrepareMap(ctx, c.ids, c.n);
   if (rc || (by_id && (rc = UploadIds(ctx, c.ids, c.n, &c.d_ids)))) return rc;
   const bool host = c.host.packets_in || c.host.packets_out;
@@ -788,9 +824,10 @@ int RunCodecCall(lyra_b200_ctx* ctx, CodecCall c) {
   }
   const CodecCall::Io& h = c.host;
   const lyra_b200_ctx::GraphKey key =
-      encoder ? lyra_b200_ctx::GraphKey{kEncode, c.n, c.num_bits, 0, ctx->nsplit, h.pcm_in, h.packets_out, nullptr, ctx->rate_override}
+      encoder ? lyra_b200_ctx::GraphKey{kEncode, c.n, c.num_bits, 0, ctx->nsplit, h.pcm_in, h.packets_out, nullptr, ctx->rate_override,
+                                        ctx->own_bits[r] != 0}
               : lyra_b200_ctx::GraphKey{kDecode, c.n, c.num_bits, ctx->decoder_mode, ctx->nsplit, h.packets_in, h.received, h.pcm_out,
-                                        ctx->rate_override};
+                                        ctx->rate_override, ctx->own_bits[r] != 0};
   const bool graphed = host && (c.kind == kEncode || c.kind == kDecode) && c.ids == nullptr && ctx->map_dense_n == c.n;
   if ((rc = RunMaybeGraphed(ctx, key, graphed, [&]() {
          return encoder ? RunEncode(ctx, c) : c.kind == kDecodePlc ? RunDecodePlc(ctx, c) : RunDecode(ctx, c);
@@ -798,7 +835,10 @@ int RunCodecCall(lyra_b200_ctx* ctx, CodecCall c) {
     return rc;
   if (!host) return LYRA_B200_OK;
   CU(SyncStream(ctx));
-  for (int k = 0; k < c.n && c.packet_bytes; ++k) c.packet_bytes[k] = dtx_flags[(size_t)k] ? 0 : PacketBytes(c.num_bits);
+  for (int k = 0; k < c.n && c.packet_bytes; ++k) {
+    const int b = own[(size_t)(c.ids ? c.ids[k] : k)];
+    c.packet_bytes[k] = dtx_flags[(size_t)k] ? 0 : PacketBytes(b ? b : c.num_bits);
+  }
   return LYRA_B200_OK;
 }
 
@@ -860,6 +900,8 @@ const char* RecordProblem(const lyra_b200_ctx* ctx, const uint8_t* rec) {
       return "decoder control state out of range";
     if (check == lyra_b200_ctx::kCheckStreamRate && RecordWord(rec, w0) != 0 && !StreamRateOk(ctx, (int32_t)RecordWord(rec, w0)))
       return "stream sample rate unsupported or above the context's";
+    if (check == lyra_b200_ctx::kCheckStreamBits && RecordWord(rec, w0) != 0 && !StreamBitsOk(ctx, (int32_t)RecordWord(rec, w0)))
+      return "stream bit count is not a multiple of 4 in 4..184";
   }
   return nullptr;
 }
@@ -907,22 +949,33 @@ int CopyStreamState(lyra_b200_ctx* ctx, const StreamStateTable& T, const int32_t
   return LYRA_B200_OK;
 }
 
-// StreamRateKernel on ctx->stream, one launch per kStateChunk streams: stream ids[k] (nullptr: k) <- rates[k] (nullptr: the
-// context's rate).  Ids and rates travel as kernel parameters.
-int LaunchStreamRates(lyra_b200_ctx* ctx, const int32_t* ids, int n, const int32_t* rates) {
+// StreamRateKernel on ctx->stream, one launch per kStateChunk streams: word[ids[k]] (ids nullptr: k) <- values[k] (nullptr:
+// ctx_value), stored as 0 when it equals ctx_value; conv0 / conv1 as in StreamRateKernel.  Ids and values travel as kernel
+// parameters.  The sample rates: (ctx->sample_rate, d_stream_rate, the codec converters); the bit counts: (0, d_stream_bits[r],
+// none).
+int LaunchStreamWords(lyra_b200_ctx* ctx, const int32_t* ids, int n, const int32_t* values, int ctx_value, int* word, int* conv0 = nullptr,
+                      int* conv1 = nullptr) {
   StreamRateChunk c;
   for (int k0 = 0; k0 < n; k0 += kStateChunk) {
     c.n = n - k0 < kStateChunk ? n - k0 : kStateChunk;
     for (int k = 0; k < c.n; ++k) {
       c.ids[k] = ids ? ids[k0 + k] : k0 + k;
-      c.rates[k] = rates ? rates[k0 + k] : ctx->sample_rate;
+      c.rates[k] = values ? values[k0 + k] : ctx_value;
     }
     if (int rc = LAUNCH(kNoProf, StreamRateKernel, dim3((unsigned)((c.n + kStreamRateThreads - 1) / kStreamRateThreads)),
-                        dim3(kStreamRateThreads), (size_t)0, ctx->stream,
-                        c, ctx->sample_rate, ctx->d_stream_rate, ctx->d_codec_rs_pos[0], ctx->d_codec_rs_pos[1]))
+                        dim3(kStreamRateThreads), (size_t)0, ctx->stream, c, ctx_value, word, conv0, conv1))
       return rc;
   }
   return LYRA_B200_OK;
+}
+int LaunchStreamRates(lyra_b200_ctx* ctx, const int32_t* ids, int n, const int32_t* rates) {
+  return LaunchStreamWords(ctx, ids, n, rates, ctx->sample_rate, ctx->d_stream_rate, ctx->d_codec_rs_pos[0], ctx->d_codec_rs_pos[1]);
+}
+
+// role index of a role that must be exactly one role of the context (0 encoder, 1 decoder), or -1 with ctx->err set
+int BitsRole(lyra_b200_ctx* ctx, int role) {
+  if (role != LYRA_B200_ROLE_ENCODER && role != LYRA_B200_ROLE_DECODER) { ctx->err = "role must be LYRA_B200_ROLE_ENCODER or _DECODER"; return -1; }
+  return RoleOk(ctx, role) ? role - 1 : -1;
 }
 
 }  // namespace
@@ -1020,6 +1073,13 @@ int lyra_b200_create_ex(const char* model_dir, int device, int max_streams, int 
     ok = ok && DevStreamState(ctx, &ctx->d_codec_rs_delay[d], (size_t)(kResamplerTaps - 1));
     ok = ok && DevStreamState(ctx, &ctx->d_codec_rs_pos[d], 2, nullptr, d == 0 ? kStateCodecRs0 : kStateCodecRs1,
                               lyra_b200_ctx::kCheckResamplerPos);
+  }
+  // the stream's own bit count per role (lyra_b200_set_stream_bits): 0, the call's, at creation and after reset
+  // (registered before the rate word, which stays the last word of a record)
+  for (int r = 0; r < 2; ++r) {
+    if (!(roles & (r + 1))) continue;
+    ok = ok && DevStreamState(ctx, &ctx->d_stream_bits[r], 1, nullptr, kStatePlain, lyra_b200_ctx::kCheckStreamBits);
+    ctx->bits_mirror[r].assign((size_t)max_streams, 0);
   }
   // the stream's own sample rate (lyra_b200_set_stream_sample_rates): 0, the context's, at creation and after reset
   ok = ok && DevStreamState(ctx, &ctx->d_stream_rate, 1, nullptr, kStatePlain, lyra_b200_ctx::kCheckStreamRate);
@@ -1123,6 +1183,8 @@ int lyra_b200_reset(lyra_b200_ctx* ctx, const int32_t* stream_ids, int n) {
     n = (int)distinct.size();
   }
   if ((rc = CopyStreamState(ctx, ctx->reset_table, nullptr, stream_ids, n))) return rc;
+  for (int r = 0; r < 2; ++r)
+    for (int k = 0; k < n && ctx->own_bits[r]; ++k) SetMirrorBits(ctx, r, stream_ids ? stream_ids[k] : k, 0);
   CU(SyncStream(ctx));
   return LYRA_B200_OK;
 }
@@ -1242,6 +1304,41 @@ int lyra_b200_stream_sample_rates(lyra_b200_ctx* ctx, const int32_t* stream_ids,
 }
 
 int lyra_b200_sample_rate(const lyra_b200_ctx* ctx) { return ctx ? ctx->sample_rate : LYRA_B200_EINVAL; }
+
+int lyra_b200_set_stream_bits(lyra_b200_ctx* ctx, int role, const int32_t* stream_ids, int n, const int32_t* bits) {
+  if (!ctx || !bits) return LYRA_B200_EINVAL;
+  ENTER(0);
+  const int r = BitsRole(ctx, role);
+  if (r < 0) return LYRA_B200_EINVAL;
+  int rc = CheckIds(ctx, stream_ids, n, false);
+  if (rc) return rc;
+  bool changes = false;
+  for (int k = 0; k < n; ++k) {
+    if (bits[k] != 0 && !StreamBitsOk(ctx, bits[k])) {
+      ctx->err = "a stream's own bit count is 0 (the call's) or a multiple of 4 in 4..184";
+      return LYRA_B200_EINVAL;
+    }
+    changes |= ctx->bits_mirror[r][(size_t)(stream_ids ? stream_ids[k] : k)] != bits[k];
+  }
+  if (!changes) return LYRA_B200_OK;
+  if ((rc = LaunchStreamWords(ctx, stream_ids, n, bits, 0, ctx->d_stream_bits[r]))) return rc;
+  for (int k = 0; k < n; ++k) SetMirrorBits(ctx, r, stream_ids ? stream_ids[k] : k, bits[k]);
+  return LYRA_B200_OK;
+}
+
+int lyra_b200_stream_bits(lyra_b200_ctx* ctx, int role, const int32_t* stream_ids, int n, int32_t* bits) {
+  if (!ctx || !bits) return LYRA_B200_EINVAL;
+  ENTER(0);
+  const int r = BitsRole(ctx, role);
+  if (r < 0) return LYRA_B200_EINVAL;
+  const int rc = CheckIds(ctx, stream_ids, n, true);
+  if (rc) return rc;
+  CU(SyncStream(ctx));
+  std::vector<int> words((size_t)ctx->max_streams);
+  CU(cudaMemcpy(words.data(), ctx->d_stream_bits[r], sizeof(int) * words.size(), cudaMemcpyDeviceToHost));
+  for (int k = 0; k < n; ++k) bits[k] = words[(size_t)(stream_ids ? stream_ids[k] : k)];
+  return LYRA_B200_OK;
+}
 
 int lyra_b200_synchronize(lyra_b200_ctx* ctx) {
   if (!ctx) return LYRA_B200_EINVAL;
@@ -1582,6 +1679,13 @@ int lyra_b200_import_streams(lyra_b200_ctx* ctx, const int32_t* stream_ids, int 
   }
   if ((rc = EnsureRecordStaging(ctx))) return rc;
   if (own_rate) ctx->rate_override = true;
+  for (size_t i = 0; i < ctx->state_list.size(); ++i) {      // the bits words' host mirror
+    const StreamStateEntry& e = ctx->state_list[i].e;
+    for (int r = 0; r < 2; ++r)
+      if (e.state == reinterpret_cast<uint32_t*>(ctx->d_stream_bits[r]))
+        for (int k = 0; k < n; ++k)
+          SetMirrorBits(ctx, r, stream_ids ? stream_ids[k] : k, (int32_t)RecordWord(recs + rb * (size_t)k, kStateHeaderWords + e.offset));
+  }
   StreamIdChunk ids;
   for (int k0 = 0; k0 < n; k0 += ctx->records_chunk) {
     ids.n = n - k0 < ctx->records_chunk ? n - k0 : ctx->records_chunk;
@@ -1598,8 +1702,12 @@ int lyra_b200_import_streams(lyra_b200_ctx* ctx, const int32_t* stream_ids, int 
 int lyra_b200_copy_streams(lyra_b200_ctx* ctx, const int32_t* src_ids, const int32_t* dst_ids, int n) {
   if (!ctx || !src_ids || !dst_ids) return LYRA_B200_EINVAL;
   ENTER(0);
-  const int rc = CheckCopyIds(ctx, src_ids, dst_ids, n);
-  return rc ? rc : CopyStreamState(ctx, ctx->state_table, src_ids, dst_ids, n);
+  int rc = CheckCopyIds(ctx, src_ids, dst_ids, n);
+  if (rc || (rc = CopyStreamState(ctx, ctx->state_table, src_ids, dst_ids, n))) return rc;
+  for (int r = 0; r < 2; ++r)                      // sources and destinations are disjoint
+    for (int k = 0; k < n && ctx->d_stream_bits[r]; ++k)
+      SetMirrorBits(ctx, r, dst_ids[k], src_ids[k] < 0 ? 0 : ctx->bits_mirror[r][(size_t)src_ids[k]]);
+  return LYRA_B200_OK;
 }
 
 int lyra_b200_noise_estimate(lyra_b200_ctx* ctx, const int32_t* ids, int n, float* noise_estimate, uint8_t* is_noise) {

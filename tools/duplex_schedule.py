@@ -21,10 +21,10 @@ def _row(t, g, m):
 
 
 class Schedule:
-    def __init__(self, slots, groups, split, mode, bits=64, rate=16000, stream_rates=None, masks=None, keep_hops=0):
+    def __init__(self, slots, groups, split, mode, bits=64, rate=16000, stream_rates=None, masks=None, keep_hops=0, stream_bits=None):
         """slots: NBUF host arrays of n rows, the input PCM (rate // 50 samples per row), or with `masks` (the decode_plc
         workload) the packets; masks: NBUF received masks of n entries.  stream_rates: the per-stream rates of every group's
-        m streams.  keep_hops: hop i < keep_hops writes its own output (and flag) buffer and keeps a copy of its packets, and
+        m streams; stream_bits: their per-stream bit counts (both roles, at most `bits`).  keep_hops: hop i < keep_hops writes its own output (and flag) buffer and keeps a copy of its packets, and
         the schedule runs at most keep_hops hops; with 0 every hop writes one shared output."""
         n = len(slots[0])
         self.n, self.m, self.bits, self.keep_hops = n, n // groups, bits, keep_hops
@@ -54,6 +54,8 @@ class Schedule:
                 c.set_split(split)
                 if stream_rates is not None:
                     c.set_stream_sample_rates(stream_rates)
+                if stream_bits is not None:
+                    c.set_stream_bits("encoder" if c is e_ else "decoder", stream_bits)
             d_.set_decoder_mode(mode)
             self.groups.append((e_, d_, gx, gy))
         self.ev_pk = [[torch.cuda.Event() for _ in range(NBUF)] for _ in range(groups)]      # [group][slot] packets written

@@ -6,14 +6,21 @@ run in one process so that clock and thermal drift hit them alike:
                      (lyra_b200_set_stream_sample_rates) so that every tile mixes the four rates;
   split              the same traffic split by rate: one context pair per rate with a quarter of the streams each (what a
                      server without per-stream rates runs);
+  bits-184           every stream at 184 bits (9.2 kbps) in --groups pairs called at 184 bits;
+  bits-mixed         --groups pairs called at 184 bits, the streams at 64 / 120 / 184 bits interleaved
+                     (lyra_b200_set_stream_bits) so that every tile and every RVQ block mixes them;
+  bits-split         the same traffic split by bit rate: one context pair per bit rate with a tile-aligned third of the streams
+                     each (what a server without per-stream bit rates runs);
   mixed-counters     16k with the odd lanes of every context set back to their state at creation (copy_streams from -1) after
                      the warm-up, so odd and even lanes stay 10 hops apart and every tile takes the per-stream hop-counter path
                      of the depthwise convolutions instead of the shared-counter fast path.
 Prints one line per run, then every configuration's median, spread and ratio to the first configuration, the card's name,
 power limit and median SM clock over the timed runs, and a JSON line.  --profile-hops adds a torch.profiler pass per
-configuration, separate from the timed runs: ResampleKernel's mean device time per launch.
+configuration, separate from the timed runs: the mean device time per launch of ResampleKernel, RvqEncodeKernel and
+RvqDecodeKernel.
 
-  python tools/schedule_bench.py [--configs 16k,48k,8k,mixed,split,mixed-counters] [--streams 4096] [--hops 200] [--runs 5]
+  python tools/schedule_bench.py [--configs 16k,48k,8k,mixed,split,bits-184,bits-mixed,bits-split,mixed-counters] [--streams 4096]
+                                 [--hops 200] [--runs 5]
 """
 import argparse
 import json
@@ -30,7 +37,9 @@ import bench  # noqa: E402
 import duplex_schedule as ds  # noqa: E402
 
 RATES = (8000, 16000, 32000, 48000)
-CONFIGS = ("16k", "8k", "32k", "48k", "mixed", "split", "mixed-counters")
+BIT_RATES = (64, 120, 184)
+CONFIGS = ("16k", "8k", "32k", "48k", "mixed", "split", "bits-184", "bits-mixed", "bits-split", "mixed-counters")
+PROFILED = ("ResampleKernel", "RvqEncodeKernel", "RvqDecodeKernel")
 
 
 def power_limit():
@@ -44,12 +53,21 @@ def power_limit():
 
 def make(name, args):
     """The schedules of one configuration."""
-    def sched(n, groups, rate=16000, stream_rates=None):
+    def sched(n, groups, rate=16000, stream_rates=None, bits=None, stream_bits=None):
         rng = np.random.default_rng(1234)
         pcm = [rng.integers(-8192, 8192, size=(n, rate // 50), dtype=np.int16) for _ in range(ds.NBUF)]
-        return ds.Schedule(pcm, groups, args.split, args.decoder_mode, args.bits, rate=rate, stream_rates=stream_rates)
+        return ds.Schedule(pcm, groups, args.split, args.decoder_mode, bits or args.bits, rate=rate, stream_rates=stream_rates,
+                           stream_bits=stream_bits)
 
     n, g = args.streams, args.groups
+    if name == "bits-184":
+        return [sched(n, g, bits=184)]
+    if name == "bits-mixed":
+        return [sched(n, g, bits=184, stream_bits=np.array([BIT_RATES[k % len(BIT_RATES)] for k in range(n // g)], dtype=np.int32))]
+    if name == "bits-split":
+        t = 8                                        # lyra_b200_tile_streams
+        cut = [0, (n // 3) // t * t, (2 * n // 3) // t * t, n]
+        return [sched(cut[i + 1] - cut[i], 1, bits=b) for i, b in enumerate(BIT_RATES)]
     if name == "mixed":
         return [sched(n, g, 48000, np.array([RATES[k % len(RATES)] for k in range(n // g)], dtype=np.int32))]
     if name == "split":
@@ -57,15 +75,19 @@ def make(name, args):
     return [sched(n, g, 16000 if name == "mixed-counters" else int(name[:-1]) * 1000)]
 
 
-def resample_kernel_us(scheds, hops):
-    """Mean device time of one ResampleKernel launch (torch.profiler, CUDA activity) over `hops` hops, and the launch count."""
+def kernel_us(scheds, hops):
+    """{kernel: (mean device time of one launch, launch count)} of the PROFILED kernels (torch.profiler, CUDA activity) over
+    `hops` hops."""
     from torch.profiler import ProfilerActivity, profile
     torch.cuda.synchronize()
     with profile(activities=[ProfilerActivity.CUDA]) as prof:
         ds.run(scheds, hops)
         torch.cuda.synchronize()
-    times = [ev.time_range.elapsed_us() for ev in prof.events() if "ResampleKernel" in ev.name]
-    return (sum(times) / len(times) if times else None), len(times)
+    res = {}
+    for k in PROFILED:
+        times = [ev.time_range.elapsed_us() for ev in prof.events() if k in ev.name]
+        res[k] = {"us_per_launch": sum(times) / len(times) if times else None, "launches": len(times)}
+    return res
 
 
 def main():
@@ -78,7 +100,7 @@ def main():
     ap.add_argument("--split", type=int, default=2)
     ap.add_argument("--bits", type=int, default=64, help="64 bits per 20 ms hop = 3.2 kbps")
     ap.add_argument("--decoder-mode", default="tensor", choices=["exact", "tensor"])
-    ap.add_argument("--profile-hops", type=int, default=0, help="hops of the ResampleKernel profiler pass (0: none)")
+    ap.add_argument("--profile-hops", type=int, default=0, help="hops of the per-kernel profiler pass (0: none)")
     args = ap.parse_args()
     names = args.configs.split(",")
     bad = [k for k in names if k not in CONFIGS]
@@ -109,8 +131,7 @@ def main():
     kernel = {}
     if args.profile_hops:
         for k, scheds in configs.items():
-            us, count = resample_kernel_us(scheds, args.profile_hops)
-            kernel[k] = {"us_per_launch": us, "launches": count}
+            kernel[k] = kernel_us(scheds, args.profile_hops)
     for scheds in configs.values():
         for s in scheds:
             s.close()
@@ -120,14 +141,15 @@ def main():
         "gpu": torch.cuda.get_device_name(), "power_limit": power_limit(), "clocks": clocks, "streams": args.streams,
         "bits": args.bits, "decoder_mode": args.decoder_mode, "split": args.split, "groups": args.groups, "hops_per_run": args.hops,
         "frames_per_s": fps, "median_frames_per_s": med, "spread": {k: [min(v) / med[k], max(v) / med[k]] for k, v in fps.items()},
-        "ratio_to_" + base: {k: v / med[base] for k, v in med.items()}, "resample_kernel": kernel,
+        "ratio_to_" + base: {k: v / med[base] for k, v in med.items()}, "kernels": kernel,
     }
     for k in names:
         print("%-14s: median %.3f M frames/s (runs %.3f-%.3f), %.3f x %s" % (k, med[k] / 1e6, min(fps[k]) / 1e6, max(fps[k]) / 1e6,
                                                                          med[k] / med[base], base))
-    for k, v in kernel.items():
-        if v["launches"]:
-            print("ResampleKernel in %s: %.1f us per launch (%d launches)" % (k, v["us_per_launch"], v["launches"]))
+    for k, per in kernel.items():
+        for name, v in per.items():
+            if v["launches"]:
+                print("%s in %s: %.1f us per launch (%d launches)" % (name, k, v["us_per_launch"], v["launches"]))
     print("GPU %s, power limit %s, median SM clock %s MHz" % (res["gpu"], res["power_limit"], clocks["sm_mhz"]))
     print(json.dumps(res))
 
