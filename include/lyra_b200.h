@@ -91,6 +91,17 @@ int lyra_b200_import_streams(lyra_b200_ctx* ctx, const int32_t* stream_ids, int 
  * excepted) or within dst_ids, or an id that is both a source and a destination.  With it a server keeps its live calls on
  * streams 0..n-1 of the *_device calls: when the call on stream h ends it copies stream n-1 into h and shrinks n. */
 int lyra_b200_copy_streams(lyra_b200_ctx* ctx, const int32_t* src_ids, const int32_t* dst_ids, int n);
+/* Afterwards each network hop counter of stream stream_ids[k] equals the matching counter of stream like_ids[k] (-1: counter 0,
+ * the phase at creation): encoder entries in a context with the encoder role, decoder entries in one with the decoder role.
+ * The stream's depthwise rings are rotated to match, so its later outputs (packets, PCM, comfort-noise flags, control state, in
+ * both decoder modes) are bit-identical to what it would have produced without the call; every other piece of its state stays
+ * as it is.  A hop counter only decides where each ring starts, but the conv-net kernels take their fast depthwise path only
+ * on a tile whose active streams share one counter: a server aligns a moved or newly admitted stream like a live neighbour
+ * of its tile, and may periodically align a whole tile to one of its lanes (streams that sit out hops, DTX or comfort noise,
+ * fall behind their neighbours).  n == 0 does nothing.  LYRA_B200_EINVAL, with nothing queued or changed, for a NULL list
+ * with n > 0, ids out of range, a repeated id within stream_ids, or an id in both lists; like_ids may repeat.  Asynchronous
+ * like lyra_b200_copy_streams: queued on the installed stream, no host synchronisation, captured graphs stay valid. */
+int lyra_b200_align_streams(lyra_b200_ctx* ctx, const int32_t* stream_ids, const int32_t* like_ids, int n);
 
 /* ---- fused codec calls: host buffers in, host buffers out ------------------------------------------ */
 

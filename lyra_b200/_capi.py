@@ -86,6 +86,7 @@ class CApi:
             "lyra_b200_export_streams": (ci, [vp, vp, ci, vp]),
             "lyra_b200_import_streams": (ci, [vp, vp, ci, vp]),
             "lyra_b200_copy_streams": (ci, [vp, vp, vp, ci]),
+            "lyra_b200_align_streams": (ci, [vp, vp, vp, ci]),
         }
         for name, (res, args) in sig.items():
             fn = getattr(L, name)   # AttributeError here = the library does not export the declared ABI
@@ -105,7 +106,7 @@ class CApi:
                "lyra_b200_encode_dtx", "lyra_b200_encode_dtx_device", "lyra_b200_resample", "lyra_b200_set_sample_rate",
                "lyra_b200_sample_rate", "lyra_b200_set_stream_sample_rates", "lyra_b200_stream_sample_rates", "lyra_b200_set_stream_bits",
                "lyra_b200_stream_bits", "lyra_b200_stream_state_bytes", "lyra_b200_export_streams", "lyra_b200_import_streams",
-               "lyra_b200_copy_streams"]
+               "lyra_b200_copy_streams", "lyra_b200_align_streams"]
 
 
 _product = None
@@ -213,6 +214,15 @@ class Context:
         if src.size != dst.size:
             raise ValueError("src_ids and dst_ids must have the same length")
         self._check(self.api.lib.lyra_b200_copy_streams(self.h, _ptr(src), _ptr(dst), src.size))
+
+    def align_streams(self, stream_ids, like_ids):
+        """Stream stream_ids[k] takes the network hop counters of stream like_ids[k] (-1: those at creation) and computes exactly
+        what it computed before; asynchronous on the installed stream."""
+        ids = np.ascontiguousarray(stream_ids, dtype=np.int32).reshape(-1)
+        like = np.ascontiguousarray(like_ids, dtype=np.int32).reshape(-1)
+        if ids.size != like.size:
+            raise ValueError("stream_ids and like_ids must have the same length")
+        self._check(self.api.lib.lyra_b200_align_streams(self.h, _ptr(ids), _ptr(like), ids.size))
 
     def set_sample_rate(self, sample_rate_hz):
         """External rate of encode / decode / decode_plc / encode_dtx / decode_track_noise and their *_device twins: 8000, 16000

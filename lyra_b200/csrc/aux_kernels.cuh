@@ -2,6 +2,7 @@
 #pragma once
 
 #include "kernel_prims.cuh"
+#include "net_kernels.cuh"
 
 namespace lyra_b200 {
 
@@ -311,6 +312,81 @@ StreamStateCopyKernel(StreamStateTable T, StreamIdChunk ids) {
     }
   }
   if (e.n18 && tid < rows) e.n18[ids.dst[r0 + tid]] = ids.src[r0 + tid] < 0 ? 0 : e.n18[ids.src[r0 + tid]];
+}
+
+// ------------------------------------------------------------------------------------------------
+// lyra_b200_align_streams: stream ids.dst[k] takes the hop counter of stream ids.src[k] (-1: 0, the counter at creation) in every
+// network entry of the table, and its depthwise rings are rotated so that it computes what it computed before.  A counter only
+// places the rings: relative row r of a ring lives in slot (n T + r) mod R (kDwRings), so moving from n to m moves the content
+// of slot p to slot p + d, d = ((m - n) T) mod R.  Same grid as the state-record kernels: blockIdx.y = entry, 8 rows of the call
+// per block on 8 consecutive threads (whole 32-byte tile rows when the rows are the lanes of a tile), the other 32 threads of
+// each row walk its ring columns.  A block reads and writes only its own rows' counters and rings, and no listed stream is a
+// like stream, so blocks need no ordering between them.
+struct StreamAlignEntry {
+  uint32_t* state;               // tile-blocked [tile][units][kTileStreams]
+  int* n18;
+  int units, layout;             // layout: index w of the state layout (kDwRingFirst)
+};
+struct StreamAlignTable { StreamAlignEntry e[4]; int count; };
+
+// entry y of the table, field by field: indexing the by-value parameter with y would copy it to local memory
+__device__ __forceinline__ StreamAlignEntry PickAlignEntry(const StreamAlignTable& T, int y) {
+  StreamAlignEntry e;
+  e.state = y == 0 ? T.e[0].state : y == 1 ? T.e[1].state : y == 2 ? T.e[2].state : T.e[3].state;
+  e.n18 = y == 0 ? T.e[0].n18 : y == 1 ? T.e[1].n18 : y == 2 ? T.e[2].n18 : T.e[3].n18;
+  e.units = y == 0 ? T.e[0].units : y == 1 ? T.e[1].units : y == 2 ? T.e[2].units : T.e[3].units;
+  e.layout = y == 0 ? T.e[0].layout : y == 1 ? T.e[1].layout : y == 2 ? T.e[2].layout : T.e[3].layout;
+  return e;
+}
+
+// col[j] <- col[(j - d) mod R] for the R units of one ring column of one lane (unit stride kTileStreams); all R loads first
+// (addresses vary, register indices do not)
+template <int R>
+__device__ __forceinline__ void RotateRingColumn(uint32_t* col, int d) {
+  uint32_t v[R];
+#pragma unroll
+  for (int j = 0; j < R; ++j) v[j] = col[(j >= d ? j - d : j - d + R) * kTileStreams];
+#pragma unroll
+  for (int j = 0; j < R; ++j) col[j * kTileStreams] = v[j];
+}
+
+// rings I .. END - 1 of kDwRings for one lane (lane: its unit 0), counter n -> m; columns c0, c0 + step, ...
+template <int I, int END>
+__device__ __forceinline__ void AlignRings(uint32_t* lane, int n, int m, int c0, int step) {
+  if constexpr (I < END) {
+    constexpr DwRing g = kDwRings[I];
+    int d = ((m - n) * g.T) % g.R;
+    d += d < 0 ? g.R : 0;
+    if (d)
+      for (int c = c0; c < g.rows; c += step) RotateRingColumn<g.R>(lane + (size_t)(g.unit + c * g.R) * kTileStreams, d);
+    AlignRings<I + 1, END>(lane, n, m, c0, step);
+  }
+}
+
+__global__ void __launch_bounds__(kStateThreads)
+StreamAlignKernel(StreamAlignTable T, StreamIdChunk ids) {
+  const int r0 = (int)blockIdx.x * kStateRows, tid = (int)threadIdx.x;
+  const int rows = ids.n - r0 < kStateRows ? ids.n - r0 : kStateRows;
+  if (rows <= 0) return;
+  const StreamAlignEntry e = PickAlignEntry(T, (int)blockIdx.y);
+  const int j = tid % kStateRows, uu = tid / kStateRows;
+  int s = 0, n = 0, m = 0;
+  if (j < rows) {
+    s = ids.dst[r0 + j];
+    const int like = ids.src[r0 + j];
+    n = e.n18[s];
+    m = like < 0 ? 0 : e.n18[like];
+    uint32_t* lane = e.state + (size_t)(s / kTileStreams) * e.units * kTileStreams + s % kTileStreams;
+    constexpr int step = kStateThreads / kStateRows;
+    if (m != n) {
+      if (e.layout == 0) AlignRings<kDwRingFirst[0], kDwRingFirst[1]>(lane, n, m, uu, step);
+      else if (e.layout == 1) AlignRings<kDwRingFirst[1], kDwRingFirst[2]>(lane, n, m, uu, step);
+      else if (e.layout == 2) AlignRings<kDwRingFirst[2], kDwRingFirst[3]>(lane, n, m, uu, step);
+      else AlignRings<kDwRingFirst[3], kDwRingFirst[4]>(lane, n, m, uu, step);
+    }
+  }
+  __syncthreads();                                   // every thread of row j has read its counter
+  if (tid < rows && m != n) e.n18[s] = m;            // thread tid < 8 is row tid
 }
 
 // ------------------------------------------------------------------------------------------------

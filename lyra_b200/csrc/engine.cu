@@ -63,6 +63,7 @@ struct lyra_b200_ctx {
   // streaming state, one block per kernel
   uint32_t* d_state[4] = {nullptr, nullptr, nullptr, nullptr};
   int* d_n18[4] = {nullptr, nullptr, nullptr, nullptr};
+  StreamAlignTable align_table{};    // the network entries the context holds, as StreamAlignKernel sees them
   float* d_mid_enc = nullptr;
   float* d_mid_dec = nullptr;
   int16_t* d_logmel_prev[3] = {nullptr, nullptr, nullptr};   // banks 0/1: lyra_b200_logmel; bank 2: the noise estimator's extractor
@@ -928,6 +929,18 @@ int CheckCopyIds(lyra_b200_ctx* ctx, const int32_t* src, const int32_t* dst, int
   return LYRA_B200_OK;
 }
 
+// ids for lyra_b200_align_streams: n in [1, max_streams]; ids in [0, max_streams) and distinct, like in [-1, max_streams) (repeats
+// allowed), no id in both
+int CheckAlignIds(lyra_b200_ctx* ctx, const int32_t* ids, const int32_t* like, int n) {
+  if (int rc = CheckIds(ctx, ids, n, false)) return rc;     // marks ids with ctx->id_gen
+  for (int k = 0; k < n; ++k) {
+    const int id = like[k];
+    if (id < -1 || id >= ctx->max_streams) { ctx->err = "like stream id out of range"; return LYRA_B200_EINVAL; }
+    if (id >= 0 && ctx->id_seen[(size_t)id] == ctx->id_gen) { ctx->err = "a stream id is both aligned and a like stream"; return LYRA_B200_EINVAL; }
+  }
+  return LYRA_B200_OK;
+}
+
 // grid of a record kernel over `rows` rows of a call: 8 rows per block, one block row per entry of T (+ `extra`)
 dim3 StateGrid(const StreamStateTable& T, int rows, int extra) {
   return dim3((unsigned)((rows + kStateRows - 1) / kStateRows), (unsigned)(T.count + extra));
@@ -1033,6 +1046,7 @@ int lyra_b200_create_ex(const char* model_dir, int device, int max_streams, int 
     if (!(roles & (w < 2 ? LYRA_B200_ROLE_ENCODER : LYRA_B200_ROLE_DECODER))) continue;   // an encoder-only / decoder-only context
     ok = DevStreamState(ctx, &ctx->d_state[w], (size_t)units[w], InitImage(ctx->spec, w).data(), kStatePlain, lyra_b200_ctx::kCheckNone,
                         true, kTileStreams, &ctx->d_n18[w]);
+    ctx->align_table.e[ctx->align_table.count++] = {ctx->d_state[w], ctx->d_n18[w], units[w], w};
   }
   if (roles & LYRA_B200_ROLE_ENCODER) ok = ok && DevAlloc(ctx, &ctx->d_mid_enc, P * 128 * 4);
   if (roles & LYRA_B200_ROLE_DECODER) ok = ok && DevAlloc(ctx, &ctx->d_mid_dec, P * 128 * 4);
@@ -1707,6 +1721,28 @@ int lyra_b200_copy_streams(lyra_b200_ctx* ctx, const int32_t* src_ids, const int
   for (int r = 0; r < 2; ++r)                      // sources and destinations are disjoint
     for (int k = 0; k < n && ctx->d_stream_bits[r]; ++k)
       SetMirrorBits(ctx, r, dst_ids[k], src_ids[k] < 0 ? 0 : ctx->bits_mirror[r][(size_t)src_ids[k]]);
+  return LYRA_B200_OK;
+}
+
+int lyra_b200_align_streams(lyra_b200_ctx* ctx, const int32_t* stream_ids, const int32_t* like_ids, int n) {
+  if (!ctx) return LYRA_B200_EINVAL;
+  if (n == 0) return LYRA_B200_OK;
+  if (!stream_ids || !like_ids) { ctx->err = "stream_ids and like_ids are required"; return LYRA_B200_EINVAL; }
+  ENTER(0);
+  int rc = CheckAlignIds(ctx, stream_ids, like_ids, n);
+  if (rc) return rc;
+  const StreamAlignTable& T = ctx->align_table;
+  StreamIdChunk ids;
+  for (int k0 = 0; k0 < n; k0 += kStateChunk) {     // the ids travel as kernel parameters
+    ids.n = n - k0 < kStateChunk ? n - k0 : kStateChunk;
+    for (int k = 0; k < ids.n; ++k) {
+      ids.src[k] = like_ids[k0 + k];
+      ids.dst[k] = stream_ids[k0 + k];
+    }
+    if ((rc = LAUNCH(kNoProf, StreamAlignKernel, dim3((unsigned)((ids.n + kStateRows - 1) / kStateRows), (unsigned)T.count),
+                     dim3(kStateThreads), (size_t)0, ctx->stream, T, ids)))
+      return rc;
+  }
   return LYRA_B200_OK;
 }
 

@@ -23,11 +23,13 @@ namespace lyra_b200 {
 constexpr int kTileStreams = 8;
 
 // ---- per-tile state layouts, in 4-byte units (each unit is S lanes wide) ----
+// kT*: time rows per hop of the layers that own the rings (the T of their depthwise calls)
 struct EncStateA {
   static constexpr int kFirst = 0;                               // [48]
   static constexpr int kRing0 = 48, kRing1 = kRing0 + 64 * 2, kRing2 = kRing1 + 64 * 6;   // [64][2|6|18]
   static constexpr int kDown0 = kRing2 + 64 * 18;                // [64][5]
   static constexpr int kUnits = kDown0 + 64 * 5;                 // 2032
+  static constexpr int kT = 20;                                  // encoder_0
 };
 struct EncStateB {
   static constexpr int kRing0 = 0, kRing1 = 128 * 2, kRing2 = kRing1 + 128 * 6;           // f32 [128][2|6|18]
@@ -38,6 +40,7 @@ struct EncStateB {
   static constexpr int kDown2 = kRingQ1 + 64 * 18;               // words [64][2]
   static constexpr int kBott = kDown2 + 64 * 2;                  // words [128][2]
   static constexpr int kUnits = kBott + 128 * 2;                 // 6016
+  static constexpr int kT1 = 4, kT2 = 2;                         // encoder_1; encoder_2 (kRingM) and quant_encoder_2 (kRingQ*)
 };
 struct DecStateC {
   static constexpr int kBott = 0;                                // f32 [64][2]
@@ -48,13 +51,51 @@ struct DecStateC {
   static constexpr int kRingQ0 = kRingM + 64 * 2;                // words [64][6]
   static constexpr int kRingQ1 = kRingQ0 + 64 * 6;               // words [64][18]
   static constexpr int kUnits = kRingQ1 + 64 * 18;               // 5888
+  static constexpr int kT0 = 2, kT1 = 4;                         // quant_decoder_0 (kRingM, kRingQ*); decoder_1
 };
 struct DecStateD {
   static constexpr int kUp2 = 0;                                 // f32 [64][5]
   static constexpr int kRing0 = 320, kRing1 = kRing0 + 64 * 2, kRing2 = kRing1 + 64 * 6;  // f32 [64][2|6|18]
   static constexpr int kLast = kRing2 + 64 * 18;                 // f32 [48]
   static constexpr int kUnits = kLast + 48;                      // 2032
+  static constexpr int kT = 20;                                  // decoder_2
 };
+// The int8 residual units (ResUnitI8) run two time rows per hop: quant_encoder_2 and quant_decoder_0
+constexpr int kResI8Rows = 2;
+
+// The dilated depthwise rings of the four layouts (w = 0 EncStateA, 1 EncStateB, 2 DecStateC, 3 DecStateD: the order of the
+// network entries of a context), rings kDwRings[kDwRingFirst[w] .. kDwRingFirst[w + 1]) of layout w.  A ring is `rows`
+// columns per lane (channels; int8 rings: packed words of 4 channels) of R units from unit `unit` on, [rows][R] (RingSlot);
+// its layer runs T rows per hop, so a stream at hop counter n keeps relative row r in slot (n T + r) mod R.
+// StreamAlignKernel (aux_kernels.cuh) rotates them.
+struct DwRing { int unit, rows, R, T; };
+constexpr DwRing kDwRings[] = {
+    {EncStateA::kRing0, 64, 2, EncStateA::kT},  {EncStateA::kRing1, 64, 6, EncStateA::kT},  {EncStateA::kRing2, 64, 18, EncStateA::kT},
+    {EncStateB::kRing0, 128, 2, EncStateB::kT1}, {EncStateB::kRing1, 128, 6, EncStateB::kT1}, {EncStateB::kRing2, 128, 18, EncStateB::kT1},
+    {EncStateB::kRingM, 256, 2, EncStateB::kT2}, {EncStateB::kRingQ0, 64, 6, EncStateB::kT2}, {EncStateB::kRingQ1, 64, 18, EncStateB::kT2},
+    {DecStateC::kRing0, 128, 2, DecStateC::kT1}, {DecStateC::kRing1, 128, 6, DecStateC::kT1}, {DecStateC::kRing2, 128, 18, DecStateC::kT1},
+    {DecStateC::kRingM, 64, 2, DecStateC::kT0},  {DecStateC::kRingQ0, 64, 6, DecStateC::kT0}, {DecStateC::kRingQ1, 64, 18, DecStateC::kT0},
+    {DecStateD::kRing0, 64, 2, DecStateD::kT},  {DecStateD::kRing1, 64, 6, DecStateD::kT},  {DecStateD::kRing2, 64, 18, DecStateD::kT},
+};
+constexpr int kDwRingFirst[5] = {0, 3, 9, 15, 18};
+static_assert(sizeof(kDwRings) / sizeof(kDwRings[0]) == kDwRingFirst[4], "every ring belongs to one layout");
+// Each ring is exactly the block its layout reserves: it ends where the next field starts.
+static_assert(EncStateA::kRing1 == EncStateA::kRing0 + 64 * 2 && EncStateA::kRing2 == EncStateA::kRing1 + 64 * 6 &&
+              EncStateA::kDown0 == EncStateA::kRing2 + 64 * 18, "EncStateA rings");
+static_assert(EncStateB::kRing1 == EncStateB::kRing0 + 128 * 2 && EncStateB::kRing2 == EncStateB::kRing1 + 128 * 6 &&
+              EncStateB::kDown1 == EncStateB::kRing2 + 128 * 18 && EncStateB::kRingQ0 == EncStateB::kRingM + 256 * 2 &&
+              EncStateB::kRingQ1 == EncStateB::kRingQ0 + 64 * 6 && EncStateB::kDown2 == EncStateB::kRingQ1 + 64 * 18, "EncStateB rings");
+static_assert(DecStateC::kRing1 == DecStateC::kRing0 + 128 * 2 && DecStateC::kRing2 == DecStateC::kRing1 + 128 * 6 &&
+              DecStateC::kRingM == DecStateC::kRing2 + 128 * 18 && DecStateC::kRingQ0 == DecStateC::kRingM + 64 * 2 &&
+              DecStateC::kRingQ1 == DecStateC::kRingQ0 + 64 * 6 && DecStateC::kUnits == DecStateC::kRingQ1 + 64 * 18, "DecStateC rings");
+static_assert(DecStateD::kRing1 == DecStateD::kRing0 + 64 * 2 && DecStateD::kRing2 == DecStateD::kRing1 + 64 * 6 &&
+              DecStateD::kLast == DecStateD::kRing2 + 64 * 18, "DecStateD rings");
+static_assert(EncStateB::kT2 == kResI8Rows && DecStateC::kT0 == kResI8Rows, "the int8 rings' layers are ResUnitI8's");
+constexpr bool DwRingsOk(int i) {
+  return i == kDwRingFirst[4] ||
+         ((kDwRings[i].R == 2 || kDwRings[i].R == 6 || kDwRings[i].R == 18) && kDwRings[i].T > 0 && DwRingsOk(i + 1));
+}
+static_assert(DwRingsOk(0), "R = 2 x dilation (1, 3, 9) divides 18, the hop counters' modulus");
 
 struct TileIo {
   const int* tile_list;        // tiles to process, one per block
@@ -262,7 +303,7 @@ template <int S, int NT, int DIL, int PDI = kI8Pd>
 __device__ __forceinline__ void ResUnitI8(const uint8_t* blob, const ResI8& p, uint32_t* aq, int lda, int row0a,
                                           uint32_t* resq, uint32_t* dq8, uint32_t* hq, uint32_t* ring,
                                           const int* n18, const int* active, int dil_rt = DIL) {
-  constexpr int T = 2, C = 256, LD = PadLd(T * S);
+  constexpr int T = kResI8Rows, C = 256, LD = PadLd(T * S);
   constexpr int NTW = 4;
   if (n18[S] >= 0) {
     if constexpr (DIL != 0) DwI8RingFast<S, NT, C, T, DIL>(aq, lda, row0a, dq8, LD, blob, p.dw, ring, n18[S], active);
@@ -383,7 +424,7 @@ EncoderKernelA(const uint8_t* __restrict__ blob, EncoderParams P, TileIo io, con
   }
   // ---- encoder_0: three residual units, dilation 1/3/9
   static_assert(EncStateA::kRing1 == EncStateA::kRing0 + 64 * 2 && EncStateA::kRing2 == EncStateA::kRing1 + 64 * 6, "ring blocks back to back");
-  ResUnitsF32x3<S, NT, 8, L::TN, L::TN, 4, 16, 64, 20>(blob, P.r0, u, L::LDU, 5, d, 1, st + (size_t)EncStateA::kRing0 * S, n18, active, wbuf,
+  ResUnitsF32x3<S, NT, 8, L::TN, L::TN, 4, 16, 64, EncStateA::kT>(blob, P.r0, u, L::LDU, 5, d, 1, st + (size_t)EncStateA::kRing0 * S, n18, active, wbuf,
                                                        NextF32(BlobPtr<float>(blob, P.down0.w), 16, 128, 640, d, L::kStgDown));
   // carried rows for the next frame: the last 5 activated rows
   StoreCarriedRows<S, NT, 64, 5>(st, EncStateA::kDown0, u, L::LDU, 20, active);
@@ -481,7 +522,7 @@ EncoderKernelB(const uint8_t* __restrict__ blob, EncoderParams P, TileIo io, con
   __syncthreads();
   // ---- encoder_1: three residual units @128 (second 1x1 has 2 groups)
   static_assert(EncStateB::kRing1 == EncStateB::kRing0 + 128 * 2 && EncStateB::kRing2 == EncStateB::kRing1 + 128 * 6, "ring blocks back to back");
-  ResUnitsF32x3<S, NT, TM, TN, TN, L::WM4, 16, 128, 4, false, 4 * S, 1, 1, L::kStg>(
+  ResUnitsF32x3<S, NT, TM, TN, TN, L::WM4, 16, 128, EncStateB::kT1, false, 4 * S, 1, 1, L::kStg>(
       blob, P.r1, u1, L::LD1, 2, d1, 2, st + (size_t)EncStateB::kRing0 * S, n18, active, wbuf,
       NextF32(BlobPtr<float>(blob, P.down1.w), 8, 256, 256, wbuf, L::kStg));
   StoreCarriedRows<S, NT, 128, 2>(st, EncStateB::kDown1, u1, L::LD1, 4, active);
@@ -503,10 +544,10 @@ EncoderKernelB(const uint8_t* __restrict__ blob, EncoderParams P, TileIo io, con
   //      DEQUANTIZE + f32 residual, QUANTIZE, int8 LeakyReLU
   constexpr int LD2 = 2 * S;
   if (n18[S] >= 0)
-    DwF32RingFast<S, NT, 256, 2, 1>(u2, LD2, 0, d2, LD2, BlobPtr<float>(blob, P.m_dw.w), BlobPtr<float>(blob, P.m_dw.bias),
+    DwF32RingFast<S, NT, 256, EncStateB::kT2, 1>(u2, LD2, 0, d2, LD2, BlobPtr<float>(blob, P.m_dw.w), BlobPtr<float>(blob, P.m_dw.bias),
                                     st + (size_t)EncStateB::kRingM * S, n18[S], active);
   else
-    DwF32Ring<S, NT>(u2, LD2, 0, d2, LD2, 256, 2, 1, BlobPtr<float>(blob, P.m_dw.w), BlobPtr<float>(blob, P.m_dw.bias),
+    DwF32Ring<S, NT>(u2, LD2, 0, d2, LD2, 256, EncStateB::kT2, 1, BlobPtr<float>(blob, P.m_dw.w), BlobPtr<float>(blob, P.m_dw.bias),
                      st + (size_t)EncStateB::kRingM * S, n18, active);
   {
     const float* b = BlobPtr<float>(blob, P.m_pw1.bias);
@@ -701,8 +742,8 @@ DecoderKernelC(const uint8_t* __restrict__ blob, DecoderParams P, TileIo io,
   }
   __syncthreads();
   // ---- quant_decoder_0/resnet_0 (int8 body, f32 residual add)
-  if (n18[S] >= 0) DwI8RingFast<S, NT, 256, 2, 1>(aq, LQA, 1, dq8, LQ2, blob, P.m_dw, stw + (size_t)DecStateC::kRingM * S, n18[S], active);
-  else DwI8Ring<S, NT>(aq, LQA, 1, dq8, LQ2, 256, 2, 1, blob, P.m_dw, stw + (size_t)DecStateC::kRingM * S, n18, active);
+  if (n18[S] >= 0) DwI8RingFast<S, NT, 256, DecStateC::kT0, 1>(aq, LQA, 1, dq8, LQ2, blob, P.m_dw, stw + (size_t)DecStateC::kRingM * S, n18[S], active);
+  else DwI8Ring<S, NT>(aq, LQA, 1, dq8, LQ2, 256, DecStateC::kT0, 1, blob, P.m_dw, stw + (size_t)DecStateC::kRingM * S, n18, active);
   {
     const RequantLutPack epi(blob, P.m_pw1, P.m_lr1);
     GemmI8Mma<S, NT, 4, L::kI8Pd>(dq8, LQ2, 0, 1, 1, 256, 1, 2, 256, BlobPtr<uint2>(blob, P.m_pw1.w),
@@ -748,7 +789,7 @@ DecoderKernelC(const uint8_t* __restrict__ blob, DecoderParams P, TileIo io,
   }
   // ---- decoder_1: three fp32 residual units @128
   static_assert(DecStateC::kRing1 == DecStateC::kRing0 + 128 * 2 && DecStateC::kRing2 == DecStateC::kRing1 + 128 * 6, "ring blocks back to back");
-  ResUnitsF32x3<S, NT, TM, TN, TN, L::WM4, 16, 128, 4, TC, L::LD1, L::RWM, L::RWN>(
+  ResUnitsF32x3<S, NT, TM, TN, TN, L::WM4, 16, 128, DecStateC::kT1, TC, L::LD1, L::RWM, L::RWN>(
       blob, P.r1, u1, 4 * S, 0, d1, 2, st + (size_t)DecStateC::kRing0 * S, n18, active, wbuf, NoNext());
   {
     float* out = mid + (size_t)tile * 128 * 4 * S;
@@ -851,7 +892,7 @@ DecoderKernelD(const uint8_t* __restrict__ blob, DecoderParams P, TileIo io, con
   }
   // ---- decoder_2: three residual units @64, T = 20
   static_assert(DecStateD::kRing1 == DecStateD::kRing0 + 64 * 2 && DecStateD::kRing2 == DecStateD::kRing1 + 64 * 6, "ring blocks back to back");
-  ResUnitsF32x3<S, NT, 8, L::TN, L::TN, 4, 16, 64, 20>(blob, P.r2, u, L::LDU, 3, d, 1, st + (size_t)DecStateD::kRing0 * S, n18, active, wbuf,
+  ResUnitsF32x3<S, NT, 8, L::TN, L::TN, 4, 16, 64, DecStateD::kT>(blob, P.r2, u, L::LDU, 3, d, 1, st + (size_t)DecStateD::kRing0 * S, n18, active, wbuf,
                                                        NextF32(BlobPtr<float>(blob, P.last.w), 16, 16, 256));
   // ---- last_layer: TRANSPOSE_CONV K = 64, stride 16, 64 -> 1 ; T 20 -> 320 (+48 tail) ; float -> int16
   {

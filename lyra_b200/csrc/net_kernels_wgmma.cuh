@@ -308,6 +308,7 @@ DecoderKernelDW(const uint8_t* __restrict__ blob, DecoderParams P, TileIo io, co
     // (already activated: slope 1 leaves them as they are)
     {
       const float4* w4 = reinterpret_cast<const float4*>(smf + L::kDw4 / 4) + unit * 64;      // per channel {w0, w1, w2, bias}
+      static_assert(DecStateD::kT == 20, "the ring slots below are those of decoder_2's 20 rows per hop (kDwRings)");
       const int base = (n18[s] * 20) % R;                    // ring slot of this frame's row 0 for this stream
       auto dw = [&](int t, int ch) {
         if (!has_rows) return 0.0f;

@@ -13,13 +13,16 @@ run in one process so that clock and thermal drift hit them alike:
                      each (what a server without per-stream bit rates runs);
   mixed-counters     16k with the odd lanes of every context set back to their state at creation (copy_streams from -1) after
                      the warm-up, so odd and even lanes stay 10 hops apart and every tile takes the per-stream hop-counter path
-                     of the depthwise convolutions instead of the shared-counter fast path.
+                     of the depthwise convolutions instead of the shared-counter fast path;
+  aligned-counters   mixed-counters followed by align_streams(odd lanes, like = the even lane before each) on both contexts
+                     of every pair: the same streams in the same states, every tile back on one counter.
 Prints one line per run, then every configuration's median, spread and ratio to the first configuration, the card's name,
 power limit and median SM clock over the timed runs, and a JSON line.  --profile-hops adds a torch.profiler pass per
 configuration, separate from the timed runs: the mean device time per launch of ResampleKernel, RvqEncodeKernel and
 RvqDecodeKernel.
 
-  python tools/schedule_bench.py [--configs 16k,48k,8k,mixed,split,bits-184,bits-mixed,bits-split,mixed-counters] [--streams 4096]
+  python tools/schedule_bench.py [--configs 16k,48k,8k,mixed,split,bits-184,bits-mixed,bits-split,mixed-counters,aligned-counters]
+                                 [--streams 4096]
                                  [--hops 200] [--runs 5]
 """
 import argparse
@@ -38,7 +41,7 @@ import duplex_schedule as ds  # noqa: E402
 
 RATES = (8000, 16000, 32000, 48000)
 BIT_RATES = (64, 120, 184)
-CONFIGS = ("16k", "8k", "32k", "48k", "mixed", "split", "bits-184", "bits-mixed", "bits-split", "mixed-counters")
+CONFIGS = ("16k", "8k", "32k", "48k", "mixed", "split", "bits-184", "bits-mixed", "bits-split", "mixed-counters", "aligned-counters")
 PROFILED = ("ResampleKernel", "RvqEncodeKernel", "RvqDecodeKernel")
 
 
@@ -72,7 +75,7 @@ def make(name, args):
         return [sched(n, g, 48000, np.array([RATES[k % len(RATES)] for k in range(n // g)], dtype=np.int32))]
     if name == "split":
         return [sched(n // len(RATES), 1, r) for r in RATES]
-    return [sched(n, g, 16000 if name == "mixed-counters" else int(name[:-1]) * 1000)]
+    return [sched(n, g, 16000 if name.endswith("-counters") else int(name[:-1]) * 1000)]
 
 
 def kernel_us(scheds, hops):
@@ -112,12 +115,16 @@ def main():
     for scheds in configs.values():
         ds.run(scheds, ds.NBUF + 2)          # warm-up: first launches, stream maps; every stream at hop counter 10
     torch.cuda.synchronize()
-    if "mixed-counters" in configs:
-        s = configs["mixed-counters"][0]
+    for k in ("mixed-counters", "aligned-counters"):
+        if k not in configs:
+            continue
+        s = configs[k][0]
         odd = np.arange(1, s.m, 2, dtype=np.int32)
         for e_, d_, _, _ in s.groups:
             for c in (e_, d_):
                 c.copy_streams(np.full(odd.size, -1, np.int32), odd)   # odd lanes back to hop counter 0
+                if k == "aligned-counters":
+                    c.align_streams(odd, odd - 1)                      # and onto their even neighbours' counters
         torch.cuda.synchronize()
     fps = {k: [] for k in names}
     sampler = bench.ClockSampler(0, "GPU-%s" % torch.cuda.get_device_properties(0).uuid)
