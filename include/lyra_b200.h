@@ -164,6 +164,26 @@ int lyra_b200_set_stream_bits(lyra_b200_ctx* ctx, int role, const int32_t* strea
 /* bits[k] = the word of stream stream_ids[k] (NULL: k) in `role` (0: it follows the call); an id may be listed more than once.
  * Ordered on the installed stream behind the work queued there; returns when done. */
 int lyra_b200_stream_bits(lyra_b200_ctx* ctx, int role, const int32_t* stream_ids, int n, int32_t* bits);
+/* Per-stream DTX: LyraEncoder::Create's enable_dtx (lyra/lyra_encoder.cc:79-89, 131-141) per stream, so one encoder context
+ * serves DTX and non-DTX calls side by side.  enable[k] is 1 (the default, at creation) or 0 for stream stream_ids[k] (NULL:
+ * streams 0..n-1).  Only a context with the encoder role accepts these calls.
+ *   lyra_b200_encode_dtx and lyra_b200_encode_dtx_device treat a stream with 0 exactly like a LyraEncoder created with
+ *   enable_dtx = false: its encoder-side noise estimator (and that estimator's log-mel extractor) is not fed, its hop is always
+ *   encoded, its flag is 0 and its packet_bytes is ceil(b / 8), b its own bit count (lyra_b200_set_stream_bits) or the call's
+ *   num_bits.  Per-stream sample rates and bit counts apply as usual.  lyra_b200_encode and lyra_b200_encode_device ignore the
+ *   setting.
+ *   0 -> 1 restarts the stream's encoder-side estimator and its extractor's carried samples at their creation state (a fresh
+ *   NoiseEstimator::Create); 1 -> 0 leaves them as they are (they are not read while DTX is off); setting the value a stream
+ *   already has does nothing.  Networks, hop counters, converters and bit counts always carry on.
+ * enable == NULL, a value other than 0 or 1, an id out of range, a repeated id or a context without the encoder role returns
+ * LYRA_B200_EINVAL and queues or changes nothing.  Asynchronous like lyra_b200_set_stream_bits: queued on the installed stream,
+ * no host synchronisation, captured graphs stay valid.  lyra_b200_reset and copy_streams from -1 turn DTX back on; copy, export
+ * and import carry the setting.  A context in which DTX was never turned off launches exactly what it launches without this call,
+ * and turning it off changes no launch count. */
+int lyra_b200_set_stream_dtx(lyra_b200_ctx* ctx, const int32_t* stream_ids, int n, const int32_t* enable);
+/* enable[k] = the DTX setting of stream stream_ids[k] (NULL: k); an id may be listed more than once.  Ordered on the installed
+ * stream behind the work queued there; returns when done. */
+int lyra_b200_stream_dtx(lyra_b200_ctx* ctx, const int32_t* stream_ids, int n, int32_t* enable);
 
 /* LyraEncoder::Encode without DTX (lyra/lyra_encoder.cc:113-156) for n streams:
  * pcm[n][sample_rate / 50] -> packets[n][ceil(num_bits/8)] (pcm[n][320] at the default 16 kHz; lyra_b200_set_sample_rate).

@@ -82,6 +82,8 @@ class CApi:
             "lyra_b200_stream_sample_rates": (ci, [vp, vp, ci, vp]),
             "lyra_b200_set_stream_bits": (ci, [vp, ci, vp, ci, vp]),
             "lyra_b200_stream_bits": (ci, [vp, ci, vp, ci, vp]),
+            "lyra_b200_set_stream_dtx": (ci, [vp, vp, ci, vp]),
+            "lyra_b200_stream_dtx": (ci, [vp, vp, ci, vp]),
             "lyra_b200_stream_state_bytes": (ci, [vp]),
             "lyra_b200_export_streams": (ci, [vp, vp, ci, vp]),
             "lyra_b200_import_streams": (ci, [vp, vp, ci, vp]),
@@ -105,7 +107,7 @@ class CApi:
                "lyra_b200_plc_get_state", "lyra_b200_plc_set_state", "lyra_b200_cng_generate", "lyra_b200_set_cng_seed",
                "lyra_b200_encode_dtx", "lyra_b200_encode_dtx_device", "lyra_b200_resample", "lyra_b200_set_sample_rate",
                "lyra_b200_sample_rate", "lyra_b200_set_stream_sample_rates", "lyra_b200_stream_sample_rates", "lyra_b200_set_stream_bits",
-               "lyra_b200_stream_bits", "lyra_b200_stream_state_bytes", "lyra_b200_export_streams", "lyra_b200_import_streams",
+               "lyra_b200_stream_bits", "lyra_b200_set_stream_dtx", "lyra_b200_stream_dtx", "lyra_b200_stream_state_bytes", "lyra_b200_export_streams", "lyra_b200_import_streams",
                "lyra_b200_copy_streams", "lyra_b200_align_streams"]
 
 
@@ -262,6 +264,21 @@ class Context:
         n = ids.size if ids is not None else (self.max_streams if n is None else n)
         out = np.empty(n, dtype=np.int32)
         self._check(self.api.lib.lyra_b200_stream_bits(self.h, self.ROLES.get(role, role), _ptr(ids), n, _ptr(out)))
+        return out
+
+    def set_stream_dtx(self, enable, stream_ids=None):
+        """Streams `stream_ids` (default: 0..len(enable)-1) run encode_dtx with DTX on (1, the default) or off (0: every hop is
+        encoded, as LyraEncoder with enable_dtx = false).  Encoder role only.  Asynchronous on the installed stream."""
+        e = np.ascontiguousarray(enable, dtype=np.int32).reshape(-1)
+        ids = _ids(stream_ids, e.size)
+        self._check(self.api.lib.lyra_b200_set_stream_dtx(self.h, _ptr(ids), e.size, _ptr(e)))
+
+    def stream_dtx(self, stream_ids=None, n=None):
+        """The DTX setting of each listed stream (default: streams 0..n-1, n = max_streams) -> int32[n]; 1: on."""
+        ids = None if stream_ids is None else np.ascontiguousarray(stream_ids, dtype=np.int32).reshape(-1)
+        n = ids.size if ids is not None else (self.max_streams if n is None else n)
+        out = np.empty(n, dtype=np.int32)
+        self._check(self.api.lib.lyra_b200_stream_dtx(self.h, _ptr(ids), n, _ptr(out)))
         return out
 
     @property

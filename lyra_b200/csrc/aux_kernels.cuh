@@ -157,13 +157,16 @@ RvqDecodeKernel(const uint8_t* __restrict__ blob, RvqParams P, const uint8_t* __
 //                       import and copy set the offset so that the key travels with the stream.
 enum StreamStateKind { kStatePlain = 0, kStateCodecRs0 = 1, kStateCodecRs1 = 2, kStateCng = 3 };
 constexpr uint32_t kStateMagic = 0x5453594Cu;        // "LYST"
-constexpr uint32_t kStateVersion = 3;                // 2: the per-stream sample rate joined the payload; 3: the per-stream bit counts
+// 2: the per-stream sample rate joined the payload; 3: the per-stream bit counts.  The per-stream DTX word kept 3: it adds a word
+// to encoder-role records only, whose size word (kHdrBytes) already refuses the shorter records, and decoder-only records did
+// not change.
+constexpr uint32_t kStateVersion = 3;
 constexpr int kStateHeaderWords = 16;
 // header words: magic, version, record bytes, roles, sample rate, 0, model fingerprint (lo, hi), codec converter 0 / 1 live,
 // comfort-noise key (lo, hi), 0 x 4
 enum { kHdrMagic = 0, kHdrVersion, kHdrBytes, kHdrRoles, kHdrRate, kHdrZero5, kHdrModelLo, kHdrModelHi, kHdrLive0, kHdrLive1,
        kHdrKeyLo, kHdrKeyHi };
-constexpr int kStateMaxEntries = 24;                 // a context with both roles registers exactly 24: a new per-stream entry raises it
+constexpr int kStateMaxEntries = 25;                 // a context with both roles registers exactly 25: a new per-stream entry raises it
 constexpr int kStateRows = 8;                        // rows of a call per block
 constexpr int kStateChunk = 1024;                    // rows per launch (the ids travel as kernel parameters)
 constexpr int kStateThreads = 256;
@@ -524,10 +527,12 @@ __device__ __forceinline__ void Fft1024(double* re, double* im, const double2* _
 
 // S: the extractor's tables by rate; each stream uses those of StreamRate(rate_word, stream, rate) (the encoder-side DTX
 // estimator follows the stream's rate); the sets differ only in their tables, not in hop, window or FFT size.
+// dtx_off (nullptr: none; lyra_b200_set_stream_dtx, by stream id): a stream whose word is not 0 has no DTX estimator, so its
+// extractor is not fed either (no output, carried samples untouched).
 __global__ void __launch_bounds__(kLogMelThreads)
 LogMelKernel(const uint8_t* __restrict__ blob, ByRate<LogMelParams> S, const int* __restrict__ rate_word, int rate,
              const int* __restrict__ stream_ids, int n, const int16_t* __restrict__ pcm, int16_t* __restrict__ prev,
-             float* __restrict__ out, const uint8_t* __restrict__ mask, int slot_base) {
+             float* __restrict__ out, const uint8_t* __restrict__ mask, int slot_base, const int* __restrict__ dtx_off) {
   unsigned char* smem = LYRA_DYN_SMEM();
   double* re = reinterpret_cast<double*>(smem);
   double* im = re + kLogMelFftPadded;
@@ -537,6 +542,7 @@ LogMelKernel(const uint8_t* __restrict__ blob, ByRate<LogMelParams> S, const int
   if (slot >= n) return;
   if (mask && !mask[slot]) return;     // this stream's extractor is not fed this hop (its carried samples stay)
   const int stream = stream_ids ? stream_ids[slot] : slot;
+  if (dtx_off && dtx_off[stream]) return;
   const LogMelParams P = PickByRate(S, RateIndex(StreamRate(rate_word, stream, rate)));
   const int tid = (int)threadIdx.x;
   constexpr int NT = kLogMelThreads;
@@ -601,14 +607,20 @@ struct NoiseParams { int nf, hops_per_update; float max_smoothing, bound_decay; 
 constexpr int kNoiseThreads = 192;
 __host__ __device__ constexpr int NoiseStateUnits(int nf) { return 5 * nf + 4; }
 
-// S: the constants by rate, selected per stream as in LogMelKernel (every set has nf = 160 bins)
+// S: the constants by rate, selected per stream as in LogMelKernel (every set has nf = 160 bins).  dtx_off as in LogMelKernel:
+// a stream whose word is not 0 reports is_noise 0 (LyraEncoder with enable_dtx = false encodes every hop) and its state is left
+// alone - unlike a masked stream, which reports its current is_noise.
 __global__ void __launch_bounds__(kNoiseThreads)
 NoiseEstimatorKernel(ByRate<NoiseParams> S, const int* __restrict__ rate_word, int rate, const int* __restrict__ stream_ids, int n,
                      const float* __restrict__ mel, const uint8_t* __restrict__ mask, float* __restrict__ state,
-                     uint8_t* __restrict__ is_noise_out, float* __restrict__ estimate_out, int slot_base) {
+                     uint8_t* __restrict__ is_noise_out, float* __restrict__ estimate_out, int slot_base, const int* __restrict__ dtx_off) {
   const int slot = slot_base + (int)blockIdx.x;
   if (slot >= n) return;
   const int stream = stream_ids ? stream_ids[slot] : slot;
+  if (dtx_off && dtx_off[stream]) {
+    if (is_noise_out && threadIdx.x == 0) is_noise_out[slot] = 0;
+    return;
+  }
   const NoiseParams P = PickByRate(S, RateIndex(StreamRate(rate_word, stream, rate)));
   unsigned char* smem = LYRA_DYN_SMEM();
   float* cur = reinterpret_cast<float*>(smem);       // [nf]

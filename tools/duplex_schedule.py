@@ -5,7 +5,8 @@ Each group is an encoder-only and a decoder-only context of m streams, installed
 -1 / 0, over rows [g*m, (g+1)*m) of shared input, packet and output buffers.  Hop i uses slot i % 8: its encode waits until
 the slot's previous packets have been decoded, its decode waits for its packets through an event, and nothing synchronises
 the host.  The decode_plc workload runs decode_plc_device on the decoder contexts alone, over caller-supplied packets and
-received masks.
+received masks.  With `dtx` the encoders run encode_dtx_device into a flag buffer per slot, and the decoders take a DTX hop as a
+lost packet: received = 1 - flag, computed on the decoder's CUDA stream.
 """
 import numpy as np
 import torch
@@ -21,14 +22,17 @@ def _row(t, g, m):
 
 
 class Schedule:
-    def __init__(self, slots, groups, split, mode, bits=64, rate=16000, stream_rates=None, masks=None, keep_hops=0, stream_bits=None):
+    def __init__(self, slots, groups, split, mode, bits=64, rate=16000, stream_rates=None, masks=None, keep_hops=0, stream_bits=None,
+                 dtx=None):
         """slots: NBUF host arrays of n rows, the input PCM (rate // 50 samples per row), or with `masks` (the decode_plc
         workload) the packets; masks: NBUF received masks of n entries.  stream_rates: the per-stream rates of every group's
-        m streams; stream_bits: their per-stream bit counts (both roles, at most `bits`).  keep_hops: hop i < keep_hops writes its own output (and flag) buffer and keeps a copy of its packets, and
-        the schedule runs at most keep_hops hops; with 0 every hop writes one shared output."""
+        m streams; stream_bits: their per-stream bit counts (both roles, at most `bits`); dtx: their DTX settings (1 on, 0 off;
+        None: no DTX, encode_device).  keep_hops: hop i < keep_hops writes its own output (and flag) buffer and keeps a copy of
+        its packets (and DTX flags), and the schedule runs at most keep_hops hops; with 0 every hop writes one shared output."""
         n = len(slots[0])
         self.n, self.m, self.bits, self.keep_hops = n, n // groups, bits, keep_hops
         self.plc = masks is not None
+        self.dtx = dtx is not None
         dev = lambda a: torch.from_numpy(np.ascontiguousarray(a)).cuda()   # noqa: E731
         if self.plc:
             self.pks, self.masks = [dev(x) for x in slots], [dev(x) for x in masks]
@@ -36,6 +40,10 @@ class Schedule:
             self.pcm = [dev(x) for x in slots]
             self.pks = [torch.zeros((n, _capi.packet_bytes(bits)), dtype=torch.uint8, device="cuda") for _ in range(NBUF)]
             self.kept_pks = [torch.zeros_like(self.pks[0]) for _ in range(keep_hops)]
+        if self.dtx:                      # per slot: the encoders' DTX flags and the decoders' received masks made from them
+            self.dtx_flags = [torch.zeros((n,), dtype=torch.uint8, device="cuda") for _ in range(NBUF)]
+            self.received = [torch.ones((n,), dtype=torch.bool, device="cuda") for _ in range(NBUF)]     # one byte, 0 or 1
+            self.kept_flags = [torch.zeros_like(self.dtx_flags[0]) for _ in range(keep_hops)]
         outs = max(keep_hops, 1)
         self.out = [torch.full((n, rate // 50), 0x5A5A, dtype=torch.int16, device="cuda") for _ in range(outs)]
         self.flags = [torch.full((n,), 0xAA, dtype=torch.uint8, device="cuda") for _ in range(outs)] if self.plc else None
@@ -56,6 +64,8 @@ class Schedule:
                     c.set_stream_sample_rates(stream_rates)
                 if stream_bits is not None:
                     c.set_stream_bits("encoder" if c is e_ else "decoder", stream_bits)
+                if dtx is not None and c is e_:
+                    c.set_stream_dtx(dtx)
             d_.set_decoder_mode(mode)
             self.groups.append((e_, d_, gx, gy))
         self.ev_pk = [[torch.cuda.Event() for _ in range(NBUF)] for _ in range(groups)]      # [group][slot] packets written
@@ -72,13 +82,24 @@ class Schedule:
                 continue
             if i >= NBUF:
                 gx.wait_event(self.ev_free[g][b])
-            e_.encode_device(m, _row(self.pcm[b], g, m), bits, pk)
+            rows = slice(g * m, (g + 1) * m)
+            if self.dtx:
+                e_.encode_dtx_device(m, _row(self.pcm[b], g, m), bits, pk, _row(self.dtx_flags[b], g, m))
+            else:
+                e_.encode_device(m, _row(self.pcm[b], g, m), bits, pk)
             self.ev_pk[g][b].record(gx)
             gy.wait_event(self.ev_pk[g][b])
-            d_.decode_device(m, pk, 0, bits, out)
+            rec = 0
+            if self.dtx:
+                with torch.cuda.stream(gy):                # a DTX hop reaches the decoder as a lost packet
+                    torch.eq(self.dtx_flags[b][rows], 0, out=self.received[b][rows])
+                rec = _row(self.received[b], g, m)
+            d_.decode_device(m, pk, rec, bits, out)
             if self.keep_hops:
                 with torch.cuda.stream(gy):                # before the slot is reused
-                    self.kept_pks[i][g * m:(g + 1) * m].copy_(self.pks[b][g * m:(g + 1) * m])
+                    self.kept_pks[i][rows].copy_(self.pks[b][rows])
+                    if self.dtx:
+                        self.kept_flags[i][rows].copy_(self.dtx_flags[b][rows])
             self.ev_free[g][b].record(gy)
 
     def close(self):

@@ -15,13 +15,21 @@ run in one process so that clock and thermal drift hit them alike:
                      the warm-up, so odd and even lanes stay 10 hops apart and every tile takes the per-stream hop-counter path
                      of the depthwise convolutions instead of the shared-counter fast path;
   aligned-counters   mixed-counters followed by align_streams(odd lanes, like = the even lane before each) on both contexts
-                     of every pair: the same streams in the same states, every tile back on one counter.
+                     of every pair: the same streams in the same states, every tile back on one counter;
+  dtx                speech input (tests/data/sample1_16kHz.wav tiled, stream i from offset (i * 7919) mod len), the encoders
+                     running encode_dtx_device with DTX on for every stream and the decoders taking DTX hops as lost packets;
+  dtx-mixed          dtx with DTX off for every other stream (lyra_b200_set_stream_dtx), so every tile mixes the two kinds;
+  dtx-split          the same traffic split by kind: half the streams in encode_dtx_device pairs, half in encode_device pairs
+                     (what a server without per-stream DTX runs);
+  dtx-off            dtx with DTX off for every stream, to compare with 16k.
+The dtx configurations also report the fraction of DTX hops over the timed runs.
 Prints one line per run, then every configuration's median, spread and ratio to the first configuration, the card's name,
 power limit and median SM clock over the timed runs, and a JSON line.  --profile-hops adds a torch.profiler pass per
 configuration, separate from the timed runs: the mean device time per launch of ResampleKernel, RvqEncodeKernel and
 RvqDecodeKernel.
 
-  python tools/schedule_bench.py [--configs 16k,48k,8k,mixed,split,bits-184,bits-mixed,bits-split,mixed-counters,aligned-counters]
+  python tools/schedule_bench.py [--configs 16k,48k,8k,mixed,split,bits-184,bits-mixed,bits-split,mixed-counters,aligned-counters,
+                                            dtx,dtx-mixed,dtx-split,dtx-off]
                                  [--streams 4096]
                                  [--hops 200] [--runs 5]
 """
@@ -41,7 +49,8 @@ import duplex_schedule as ds  # noqa: E402
 
 RATES = (8000, 16000, 32000, 48000)
 BIT_RATES = (64, 120, 184)
-CONFIGS = ("16k", "8k", "32k", "48k", "mixed", "split", "bits-184", "bits-mixed", "bits-split", "mixed-counters", "aligned-counters")
+CONFIGS = ("16k", "8k", "32k", "48k", "mixed", "split", "bits-184", "bits-mixed", "bits-split", "mixed-counters", "aligned-counters",
+           "dtx", "dtx-mixed", "dtx-split", "dtx-off")
 PROFILED = ("ResampleKernel", "RvqEncodeKernel", "RvqDecodeKernel")
 
 
@@ -54,15 +63,35 @@ def power_limit():
         return None
 
 
+def speech_slots(streams):
+    """ds.NBUF hops of speech for the given stream indices: tests/data/sample1_16kHz.wav tiled, stream i from offset
+    (i * 7919) mod len (SURVEY.md section 8d)"""
+    import wave
+    with wave.open(os.path.join(bench.ROOT, "tests", "data", "sample1_16kHz.wav")) as w:
+        clip = np.frombuffer(w.readframes(w.getnframes()), dtype=np.int16)
+    start = (np.asarray(streams, np.int64) * 7919) % len(clip)
+    return [clip[(start[:, None] + b * 320 + np.arange(320)[None, :]) % len(clip)] for b in range(ds.NBUF)]
+
+
 def make(name, args):
     """The schedules of one configuration."""
-    def sched(n, groups, rate=16000, stream_rates=None, bits=None, stream_bits=None):
-        rng = np.random.default_rng(1234)
-        pcm = [rng.integers(-8192, 8192, size=(n, rate // 50), dtype=np.int16) for _ in range(ds.NBUF)]
+    def sched(n, groups, rate=16000, stream_rates=None, bits=None, stream_bits=None, dtx=None, speech=None):
+        if speech is None:
+            rng = np.random.default_rng(1234)
+            pcm = [rng.integers(-8192, 8192, size=(n, rate // 50), dtype=np.int16) for _ in range(ds.NBUF)]
+        else:
+            pcm = speech_slots(speech)
         return ds.Schedule(pcm, groups, args.split, args.decoder_mode, bits or args.bits, rate=rate, stream_rates=stream_rates,
-                           stream_bits=stream_bits)
+                           stream_bits=stream_bits, dtx=dtx)
 
     n, g = args.streams, args.groups
+    if name in ("dtx", "dtx-mixed", "dtx-off"):
+        m = n // g
+        dtx = {"dtx": np.ones(m, np.int32), "dtx-mixed": (np.arange(m) % 2 == 0).astype(np.int32), "dtx-off": np.zeros(m, np.int32)}[name]
+        return [sched(n, g, dtx=dtx, speech=np.arange(n))]
+    if name == "dtx-split":
+        # the streams of dtx-mixed, each kind in context pairs of its own: DTX on (the even streams) and encode_device (the odd)
+        return [sched(n // 2, g, dtx=np.ones(n // 2 // g, np.int32), speech=np.arange(0, n, 2)), sched(n // 2, g, speech=np.arange(1, n, 2))]
     if name == "bits-184":
         return [sched(n, g, bits=184)]
     if name == "bits-mixed":
@@ -135,6 +164,11 @@ def main():
             fps[k].append(v)
             print("run %d  %-14s  %.3f M frames/s" % (run, k, v / 1e6), flush=True)
     clocks = sampler.stop()
+    dtx_frac = {}
+    for k, scheds in configs.items():      # each slot holds the flags of its latest hop: the last ds.NBUF hops of the timed runs
+        if k.startswith("dtx"):
+            torch.cuda.synchronize()
+            dtx_frac[k] = sum(int(f.sum()) for s in scheds if s.dtx for f in s.dtx_flags) / (ds.NBUF * sum(s.n for s in scheds))
     kernel = {}
     if args.profile_hops:
         for k, scheds in configs.items():
@@ -148,11 +182,12 @@ def main():
         "gpu": torch.cuda.get_device_name(), "power_limit": power_limit(), "clocks": clocks, "streams": args.streams,
         "bits": args.bits, "decoder_mode": args.decoder_mode, "split": args.split, "groups": args.groups, "hops_per_run": args.hops,
         "frames_per_s": fps, "median_frames_per_s": med, "spread": {k: [min(v) / med[k], max(v) / med[k]] for k, v in fps.items()},
-        "ratio_to_" + base: {k: v / med[base] for k, v in med.items()}, "kernels": kernel,
+        "ratio_to_" + base: {k: v / med[base] for k, v in med.items()}, "kernels": kernel, "dtx_hop_fraction": dtx_frac,
     }
     for k in names:
-        print("%-14s: median %.3f M frames/s (runs %.3f-%.3f), %.3f x %s" % (k, med[k] / 1e6, min(fps[k]) / 1e6, max(fps[k]) / 1e6,
-                                                                         med[k] / med[base], base))
+        print("%-14s: median %.3f M frames/s (runs %.3f-%.3f), %.3f x %s%s" % (
+            k, med[k] / 1e6, min(fps[k]) / 1e6, max(fps[k]) / 1e6, med[k] / med[base], base,
+            ", DTX hops %.3f" % dtx_frac[k] if k in dtx_frac else ""))
     for k, per in kernel.items():
         for name, v in per.items():
             if v["launches"]:
