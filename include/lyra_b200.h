@@ -307,6 +307,25 @@ int lyra_b200_decode_plc_device(lyra_b200_ctx* ctx, int n, const uint8_t* d_pack
                                 int16_t* d_pcm, uint8_t* d_is_comfort_noise /* may be NULL */);
 int lyra_b200_encode_dtx_device(lyra_b200_ctx* ctx, int n, const int16_t* d_pcm, int num_bits, uint8_t* d_packets,
                                 uint8_t* d_is_noise /* [n], 1 = empty packet */);
+/* Streams that sit out a hop: d_active is a device buffer the caller owns (NULL uninstalls it).  Like lyra_b200_set_stream this
+ * is a host-side setting: every later encode_device, encode_dtx_device, decode_device, decode_track_noise_device and
+ * decode_plc_device reads rows [0, n) of the buffer, in stream order on the installed stream, when its kernels run - so a server
+ * rewrites the mask each hop (cudaMemcpyAsync or a kernel of its own) with no host synchronisation.  The library never writes
+ * it; the caller keeps it valid while calls that read it are queued.
+ *   A byte of 0 sits the stream out: it is exactly a LyraEncoder / LyraDecoder that is not called this hop.  None of its state
+ *   changes (networks and hop counters, both noise estimators and their extractors, packet-loss control state, comfort-noise
+ *   buffer and hop counter, both codec converters, its rate, bits and DTX words), and its PCM row, packet row and received byte
+ *   are not read.  Its output rows: encode_device an all-zero packet; encode_dtx_device an all-zero packet and d_is_noise 1
+ *   (nothing to send, as for an empty DTX packet); decode_device a zero PCM row (sample_rate / 50 samples);
+ *   decode_track_noise_device a zero PCM row and its estimator's current is_noise, without feeding it; decode_plc_device a zero
+ *   PCM row and is_comfort_noise of its unchanged state.  Any other byte runs the stream as usual.
+ *   The host-buffer calls ignore the mask (their stream_ids say which streams run), as do noise_update_device (it has its own
+ *   update mask) and the plugin-level calls.
+ * With no mask installed the calls launch exactly what they launch without it; with one they launch the same number of kernels,
+ * and an all-ones mask gives bit-identical results.  A stream that sits out falls behind its tile neighbours' hop counters, as
+ * after DTX or comfort-noise hops: lyra_b200_align_streams puts it back on a neighbour's phase.  LYRA_B200_EINVAL only for a
+ * NULL context; works in any context. */
+int lyra_b200_set_active_mask(lyra_b200_ctx* ctx, const uint8_t* d_active);
 int lyra_b200_synchronize(lyra_b200_ctx* ctx);
 /* Dense calls (stream_ids == NULL / *_device) over many tiles are cut into `parts` (1..4, default 3) sub-batches that
  * run concurrently on internal CUDA streams so partial waves of one kernel are filled by another's blocks.

@@ -75,6 +75,7 @@ class CApi:
             "lyra_b200_set_cng_seed": (ci, [vp, C.c_uint64]),
             "lyra_b200_encode_dtx": (ci, [vp, vp, ci, vp, ci, vp, vp]),
             "lyra_b200_encode_dtx_device": (ci, [vp, ci, vp, ci, vp, vp]),
+            "lyra_b200_set_active_mask": (ci, [vp, vp]),
             "lyra_b200_resample": (ci, [vp, ci, vp, ci, ci, vp, ci, vp, ci, vp]),
             "lyra_b200_set_sample_rate": (ci, [vp, ci]),
             "lyra_b200_sample_rate": (ci, [vp]),
@@ -105,7 +106,7 @@ class CApi:
                "lyra_b200_decode_track_noise_device", "lyra_b200_set_split", "lyra_b200_set_blocking_sync", "lyra_b200_set_graphs", "lyra_b200_set_priority", "lyra_b200_graph_replays", "lyra_b200_set_decoder_mode", "lyra_b200_decoder_mode", "lyra_b200_launch_count", "lyra_b200_profile_enable",
                "lyra_b200_profile_read", "lyra_b200_noise_estimate", "lyra_b200_decode_plc", "lyra_b200_decode_plc_device",
                "lyra_b200_plc_get_state", "lyra_b200_plc_set_state", "lyra_b200_cng_generate", "lyra_b200_set_cng_seed",
-               "lyra_b200_encode_dtx", "lyra_b200_encode_dtx_device", "lyra_b200_resample", "lyra_b200_set_sample_rate",
+               "lyra_b200_encode_dtx", "lyra_b200_encode_dtx_device", "lyra_b200_set_active_mask", "lyra_b200_resample", "lyra_b200_set_sample_rate",
                "lyra_b200_sample_rate", "lyra_b200_set_stream_sample_rates", "lyra_b200_stream_sample_rates", "lyra_b200_set_stream_bits",
                "lyra_b200_stream_bits", "lyra_b200_set_stream_dtx", "lyra_b200_stream_dtx", "lyra_b200_stream_state_bytes", "lyra_b200_export_streams", "lyra_b200_import_streams",
                "lyra_b200_copy_streams", "lyra_b200_align_streams"]
@@ -344,6 +345,12 @@ class Context:
     # ---- device-resident variants (raw CUDA device pointers as ints, e.g. torch.Tensor.data_ptr()) ----
     def set_stream(self, cuda_stream_ptr):
         self._check(self.api.lib.lyra_b200_set_stream(self.h, C.c_void_p(cuda_stream_ptr or 0)))
+
+    def set_active_mask(self, mask):
+        """Install the active mask of the *_device codec calls: a device pointer (int), a uint8 CUDA tensor (its data_ptr(); the
+        caller keeps it alive while calls that read it are queued) or None to uninstall.  Row k = 0: stream k sits the call out."""
+        ptr = mask.data_ptr() if hasattr(mask, "data_ptr") else mask
+        self._check(self.api.lib.lyra_b200_set_active_mask(self.h, C.c_void_p(ptr or 0)))
 
     def decode_track_noise(self, packets, num_bits, stream_ids=None, received=None):
         """decode() + noise-estimator update of the received streams on the device -> (pcm[n][320], is_noise[n])."""

@@ -31,11 +31,12 @@ __device__ __forceinline__ int RvqStages(const int* __restrict__ bits_word, cons
 }
 
 // A block runs its stage loop to the largest stage count among its slots (the codebook double buffer is shared); each slot packs
-// its own stages into the first ceil(bits / 8) bytes of its row and zeros over the rest of the row.
+// its own stages into the first ceil(bits / 8) bytes of its row and zeros over the rest of the row.  active (nullptr: every slot;
+// lyra_b200_set_active_mask): a slot whose byte is 0 gets an all-zero packet, like a skipped one.
 __global__ void __launch_bounds__(kRvqThreads)
 RvqEncodeKernel(const uint8_t* __restrict__ blob, RvqParams P, const float* __restrict__ features, int n, int nq,
                 uint8_t* __restrict__ packets, int packet_bytes, int* __restrict__ indices_out, const uint8_t* __restrict__ skip,
-                const int* __restrict__ bits_word, const int* __restrict__ stream_ids, int slot_base) {
+                const int* __restrict__ bits_word, const int* __restrict__ stream_ids, int slot_base, const uint8_t* __restrict__ active) {
   unsigned char* smem = LYRA_DYN_SMEM();
   float* cbs = reinterpret_cast<float*>(smem);                                  // [2][64][16] stage codebooks (double buffer, 16-byte aligned)
   float* rs = cbs + 2 * 1024;                                                   // [slots][64] residuals
@@ -52,7 +53,8 @@ RvqEncodeKernel(const uint8_t* __restrict__ blob, RvqParams P, const float* __re
       if (sl < n) block_nq = max(block_nq, RvqStages(bits_word, stream_ids, slot_base, sl, nq));
     }
   }
-  const bool skipped = valid && skip != nullptr && skip[slot];     // DTX: the hop was noise, its packet is empty (bytes zeroed)
+  // DTX: the hop was noise, its packet is empty (bytes zeroed); the same for a slot that sits out
+  const bool skipped = valid && ((active != nullptr && !active[slot]) || (skip != nullptr && skip[slot]));
   float* r = rs + grp * 64;
   int* idx = idxs + grp * 48;
   const float* cbt = BlobPtr<float>(blob, P.codebooks_t);
@@ -112,17 +114,23 @@ RvqEncodeKernel(const uint8_t* __restrict__ blob, RvqParams P, const float* __re
 // (lyra/residual_vector_quantizer.cc:112-168, "decode" subgraph): left-to-right sum over all 46 stages,
 // unused stages contribute codebook[0] * 0.  A stream whose packet was not received gets 64 zero
 // features (ZeroFeatureEstimator, lyra/lyra_decoder.cc:317-326).  A slot reads its stream's own stage count (RvqStages) from
-// the first ceil(bits / 8) bytes of its row, so a stream at b bits decodes bit for bit like a call at b bits.
+// the first ceil(bits / 8) bytes of its row, so a stream at b bits decodes bit for bit like a call at b bits.  active (nullptr:
+// every slot; lyra_b200_set_active_mask): a slot whose byte is 0 reads neither its packet nor its received byte and gets zeros;
+// its 320-sample row of sat_out_pcm (nullptr: none) is written as zeros here, since the decoder nets skip it.
 __global__ void __launch_bounds__(256)
 RvqDecodeKernel(const uint8_t* __restrict__ blob, RvqParams P, const uint8_t* __restrict__ packets, int packet_bytes,
                 const uint8_t* __restrict__ received, int n, int nq, float* __restrict__ features,
-                const int* __restrict__ bits_word, const int* __restrict__ stream_ids, int slot_base) {
+                const int* __restrict__ bits_word, const int* __restrict__ stream_ids, int slot_base, const uint8_t* __restrict__ active,
+                int16_t* __restrict__ sat_out_pcm) {
   const int gid = (int)(blockIdx.x * blockDim.x + threadIdx.x);
   const int slot = gid / 64, j = gid % 64;
   if (slot >= n) return;
   nq = RvqStages(bits_word, stream_ids, slot_base, slot, nq);
   float out = 0.0f;
-  if (received == nullptr || received[slot]) {
+  const bool sat_out = active != nullptr && !active[slot];
+  if (sat_out && sat_out_pcm)
+    for (int k = j; k < 320; k += 64) sat_out_pcm[(size_t)slot * 320 + k] = 0;
+  if (!sat_out && (received == nullptr || received[slot])) {
     const float* cb = BlobPtr<float>(blob, P.codebooks);
     const uint8_t* pk = packets + (size_t)slot * packet_bytes;
     for (int k = 0; k < P.num_stages; ++k) {
@@ -528,11 +536,13 @@ __device__ __forceinline__ void Fft1024(double* re, double* im, const double2* _
 // S: the extractor's tables by rate; each stream uses those of StreamRate(rate_word, stream, rate) (the encoder-side DTX
 // estimator follows the stream's rate); the sets differ only in their tables, not in hop, window or FFT size.
 // dtx_off (nullptr: none; lyra_b200_set_stream_dtx, by stream id): a stream whose word is not 0 has no DTX estimator, so its
-// extractor is not fed either (no output, carried samples untouched).
+// extractor is not fed either (no output, carried samples untouched).  active (nullptr: every slot; lyra_b200_set_active_mask, by
+// slot): a slot whose byte is 0 sits the call out - nothing is read or written for it, not even its update-mask byte.
 __global__ void __launch_bounds__(kLogMelThreads)
 LogMelKernel(const uint8_t* __restrict__ blob, ByRate<LogMelParams> S, const int* __restrict__ rate_word, int rate,
              const int* __restrict__ stream_ids, int n, const int16_t* __restrict__ pcm, int16_t* __restrict__ prev,
-             float* __restrict__ out, const uint8_t* __restrict__ mask, int slot_base, const int* __restrict__ dtx_off) {
+             float* __restrict__ out, const uint8_t* __restrict__ mask, int slot_base, const int* __restrict__ dtx_off,
+             const uint8_t* __restrict__ active) {
   unsigned char* smem = LYRA_DYN_SMEM();
   double* re = reinterpret_cast<double*>(smem);
   double* im = re + kLogMelFftPadded;
@@ -540,6 +550,7 @@ LogMelKernel(const uint8_t* __restrict__ blob, ByRate<LogMelParams> S, const int
   double* xw = mag + kLogMelFft / 2 + 1;     // [window_len, padded like the FFT buffers] windowed samples in natural order
   const int slot = slot_base + (int)blockIdx.x;     // I/O arrays are indexed by slot; a sub-batch starts at slot_base
   if (slot >= n) return;
+  if (active && !active[slot]) return;     // the stream sits this call out
   if (mask && !mask[slot]) return;     // this stream's extractor is not fed this hop (its carried samples stay)
   const int stream = stream_ids ? stream_ids[slot] : slot;
   if (dtx_off && dtx_off[stream]) return;
@@ -610,12 +621,21 @@ __host__ __device__ constexpr int NoiseStateUnits(int nf) { return 5 * nf + 4; }
 // S: the constants by rate, selected per stream as in LogMelKernel (every set has nf = 160 bins).  dtx_off as in LogMelKernel:
 // a stream whose word is not 0 reports is_noise 0 (LyraEncoder with enable_dtx = false encodes every hop) and its state is left
 // alone - unlike a masked stream, which reports its current is_noise.
+// active (nullptr: every slot; lyra_b200_set_active_mask, by slot): a slot whose byte is 0 sits the call out and its state is left
+// alone; its update-mask byte is not read.  encoder_side: it reports is_noise 1 (nothing to send, like an empty DTX packet);
+// otherwise it reports its current is_noise / noise_estimate, like a masked stream.
 __global__ void __launch_bounds__(kNoiseThreads)
 NoiseEstimatorKernel(ByRate<NoiseParams> S, const int* __restrict__ rate_word, int rate, const int* __restrict__ stream_ids, int n,
                      const float* __restrict__ mel, const uint8_t* __restrict__ mask, float* __restrict__ state,
-                     uint8_t* __restrict__ is_noise_out, float* __restrict__ estimate_out, int slot_base, const int* __restrict__ dtx_off) {
+                     uint8_t* __restrict__ is_noise_out, float* __restrict__ estimate_out, int slot_base, const int* __restrict__ dtx_off,
+                     const uint8_t* __restrict__ active, bool encoder_side) {
   const int slot = slot_base + (int)blockIdx.x;
   if (slot >= n) return;
+  const bool sat_out = active && !active[slot];
+  if (sat_out && encoder_side) {
+    if (is_noise_out && threadIdx.x == 0) is_noise_out[slot] = 1;
+    return;
+  }
   const int stream = stream_ids ? stream_ids[slot] : slot;
   if (dtx_off && dtx_off[stream]) {
     if (is_noise_out && threadIdx.x == 0) is_noise_out[slot] = 0;
@@ -635,7 +655,7 @@ NoiseEstimatorKernel(ByRate<NoiseParams> S, const int* __restrict__ rate_word, i
   float* sq = st + 3 * nf;
   float* tmp_min = st + 4 * nf;
   int* meta = reinterpret_cast<int*>(st + 5 * nf);
-  const bool feed = mask == nullptr || mask[slot] != 0;
+  const bool feed = !sat_out && (mask == nullptr || mask[slot] != 0);
   if (!feed) {
     if (is_noise_out && i == 0) is_noise_out[slot] = meta[2] ? 0 : 1;
     if (estimate_out && i < nf) estimate_out[(size_t)slot * nf + i] = est[i];

@@ -127,6 +127,9 @@ struct lyra_b200_ctx {
   float* d_melout = nullptr;
   int* d_indices = nullptr;
   int* d_ids = nullptr;
+  // lyra_b200_set_active_mask: the caller's buffer, by row of the *_device codec calls (0 = the stream sits the call out); nullptr:
+  // every stream runs and the kernels get no pointer
+  const uint8_t* d_active = nullptr;
   // tile map
   int* d_tile_list = nullptr;
   int* d_slot_of = nullptr;
@@ -370,8 +373,10 @@ struct Part {
 };
 Part WholeCall(lyra_b200_ctx* ctx, int n) { return Part{0, ctx->active_tiles, 0, n, ctx->stream}; }
 
-int LaunchEncoderNets(lyra_b200_ctx* ctx, const Part& p, const uint8_t* skip, const int16_t* d_pcm, float* d_features) {
-  const TileIo io{ctx->d_tile_list + p.tile0, ctx->d_slot_of, skip};
+// active: lyra_b200_set_active_mask's buffer by slot (nullptr: none), here and in the Launch* functions below
+int LaunchEncoderNets(lyra_b200_ctx* ctx, const Part& p, const uint8_t* skip, const int16_t* d_pcm, float* d_features,
+                      const uint8_t* active = nullptr) {
+  const TileIo io{ctx->d_tile_list + p.tile0, ctx->d_slot_of, skip, active};
   const int rc = LAUNCH(0, EncoderKernelA, dim3((unsigned)p.ntiles), dim3(EncA::NT), (size_t)EncA::kSmemBytes, p.st,
                         ctx->d_blob, ctx->spec.enc, io, d_pcm, reinterpret_cast<float*>(ctx->d_state[0]), ctx->d_n18[0], ctx->d_mid_enc);
   return rc ? rc : LAUNCH(1, EncoderKernelB, dim3((unsigned)p.ntiles), dim3(EncB::NT), (size_t)EncB::kSmemBytes, p.st,
@@ -380,28 +385,34 @@ int LaunchEncoderNets(lyra_b200_ctx* ctx, const Part& p, const uint8_t* skip, co
 
 // bits_word (nullptr: every row at num_bits) and d_ids: the per-stream bit counts of the call's streams (RvqEncodeKernel)
 int LaunchQuantize(lyra_b200_ctx* ctx, const Part& p, const float* d_features, int num_bits, uint8_t* d_packets, int* d_indices,
-                   const uint8_t* d_skip = nullptr, const int* bits_word = nullptr, const int* d_ids = nullptr) {
+                   const uint8_t* d_skip = nullptr, const int* bits_word = nullptr, const int* d_ids = nullptr,
+                   const uint8_t* active = nullptr) {
   const int nq = num_bits / ctx->spec.bits_per_stage, pb = PacketBytes(num_bits);
   const int blocks = (p.nslots + kRvqSlotsPerBlock - 1) / kRvqSlotsPerBlock;
   return LAUNCH(2, RvqEncodeKernel, dim3((unsigned)blocks), dim3(kRvqThreads), (size_t)(2 * 1024 * 4 + kRvqSlotsPerBlock * (64 * 4 + 48 * 4)), p.st,
                 ctx->d_blob, ctx->spec.rvq, d_features + (size_t)p.slot0 * 64, p.nslots, nq, d_packets + (size_t)p.slot0 * pb, pb,
-                d_indices ? d_indices + (size_t)p.slot0 * 46 : nullptr, d_skip ? d_skip + p.slot0 : nullptr, bits_word, d_ids, p.slot0);
+                d_indices ? d_indices + (size_t)p.slot0 * 46 : nullptr, d_skip ? d_skip + p.slot0 : nullptr, bits_word, d_ids, p.slot0,
+                active ? active + p.slot0 : nullptr);
 }
 
+// sat_out_pcm: the 16 kHz PCM rows by slot that the slots sitting out (active) get as zeros (nullptr: none)
 int LaunchDequantize(lyra_b200_ctx* ctx, const Part& p, const uint8_t* d_packets, const uint8_t* d_received, int num_bits, float* d_features,
-                     const int* bits_word = nullptr, const int* d_ids = nullptr) {
+                     const int* bits_word = nullptr, const int* d_ids = nullptr, const uint8_t* active = nullptr,
+                     int16_t* sat_out_pcm = nullptr) {
   const int nq = num_bits / ctx->spec.bits_per_stage, pb = PacketBytes(num_bits);
   const int blocks = (p.nslots * 64 + 255) / 256;
   return LAUNCH(3, RvqDecodeKernel, dim3((unsigned)blocks), dim3(256), (size_t)0, p.st,
                 ctx->d_blob, ctx->spec.rvq, d_packets + (size_t)p.slot0 * pb, pb, d_received ? d_received + p.slot0 : nullptr, p.nslots, nq,
-                d_features + (size_t)p.slot0 * 64, bits_word, d_ids, p.slot0);
+                d_features + (size_t)p.slot0 * 64, bits_word, d_ids, p.slot0, active ? active + p.slot0 : nullptr,
+                active && sat_out_pcm ? sat_out_pcm + (size_t)p.slot0 * 320 : nullptr);
 }
 
 // Exact mode: DecoderKernelC<false> + DecoderKernelD, fp32 FMA chains bit-exact with the oracle.  Tensor mode: DecoderKernelC<true>
 // (decoder_1's 1x1 convolutions on mma.sync TF32) + DecoderKernelDW (warpgroup MMAs, A operands and accumulators in registers;
 // net_kernels_wgmma.cuh).
-int LaunchDecoderNets(lyra_b200_ctx* ctx, const Part& p, const uint8_t* skip, const float* d_features, int16_t* d_pcm) {
-  const TileIo io{ctx->d_tile_list + p.tile0, ctx->d_slot_of, skip};
+int LaunchDecoderNets(lyra_b200_ctx* ctx, const Part& p, const uint8_t* skip, const float* d_features, int16_t* d_pcm,
+                      const uint8_t* active = nullptr) {
+  const TileIo io{ctx->d_tile_list + p.tile0, ctx->d_slot_of, skip, active};
   const bool tc = ctx->decoder_mode == LYRA_B200_DECODER_TENSOR;
   const dim3 grid((unsigned)p.ntiles);
   float* st_c = reinterpret_cast<float*>(ctx->d_state[2]);
@@ -473,29 +484,32 @@ int ForEachPart(lyra_b200_ctx* ctx, int n, Fn body) {
 // S: the extractor's tables by rate, used per stream at StreamRate(rate_word, stream, rate) (one set: Uniform; the sets share
 // their sizes)
 int LaunchLogMel(lyra_b200_ctx* ctx, cudaStream_t st, const ByRate<LogMelParams>& S, const int* rate_word, int rate, const int* d_ids,
-                 int slot0, int count, int n, const int16_t* d_pcm, int16_t* carried, const uint8_t* d_mask, const int* dtx_off = nullptr) {
+                 int slot0, int count, int n, const int16_t* d_pcm, int16_t* carried, const uint8_t* d_mask, const int* dtx_off = nullptr,
+                 const uint8_t* active = nullptr) {
   const LogMelParams& P = S.p[0];
   const size_t smem = sizeof(double) * (size_t)(2 * kLogMelFftPadded + P.fft / 2 + 1 + P.window_len + P.window_len / 8 + 1);
   return LAUNCH(6, LogMelKernel, dim3((unsigned)count), dim3(kLogMelThreads), smem, st,
-                ctx->d_blob, S, rate_word, rate, d_ids, n, d_pcm, carried, ctx->d_melout, d_mask, slot0, dtx_off);
+                ctx->d_blob, S, rate_word, rate, d_ids, n, d_pcm, carried, ctx->d_melout, d_mask, slot0, dtx_off, active);
 }
 
 // log-mel of this hop (the estimator's own extractor, bank 2) + the estimator recurrences for slots
 // [slot0, slot0 + count) on stream `st`; all arrays are indexed by slot, n = total slots of the call.  The encoder side's
 // estimators are built for each stream's rate (NoiseEstimator::Create(rate, 320, 640, 160), lyra/lyra_encoder.cc:80-89) and
 // skip the streams whose DTX is off (lyra_b200_set_stream_dtx: flag 0, state untouched); the decoder side's stay at 16 kHz.
+// Streams that sit out (active) feed neither side: the encoder side reports flag 1, the decoder side its current flag.
 int LaunchNoiseUpdate(lyra_b200_ctx* ctx, cudaStream_t st, const int* d_ids, int slot0, int count, int n, const int16_t* d_pcm,
-                      const uint8_t* d_mask, uint8_t* d_is_noise, float* d_estimate, bool encoder_side = false) {
+                      const uint8_t* d_mask, uint8_t* d_is_noise, float* d_estimate, bool encoder_side = false,
+                      const uint8_t* active = nullptr) {
   float* noise_state = encoder_side ? ctx->d_noise_enc : ctx->d_noise;
   int16_t* carried = encoder_side ? ctx->d_logmel_prev_enc : ctx->d_logmel_prev[2];
   const int* rate_word = encoder_side ? ctx->d_stream_rate : nullptr;
   const int* dtx_off = encoder_side ? StreamWord(ctx, kWordDtxOff) : nullptr;
   const int rate = encoder_side ? ctx->sample_rate : 16000;
   const int rc = LaunchLogMel(ctx, st, encoder_side ? ctx->enc_logmel : Uniform(ctx->spec.logmel160), rate_word, rate, d_ids, slot0, count, n,
-                              d_pcm, carried, d_mask, dtx_off);
+                              d_pcm, carried, d_mask, dtx_off, active);
   return rc ? rc : LAUNCH(7, NoiseEstimatorKernel, dim3((unsigned)count), dim3(kNoiseThreads), sizeof(float) * (size_t)(2 * 160 + 2), st,
                           encoder_side ? ctx->enc_noise_params : Uniform(ctx->noise_params), rate_word, rate, d_ids, n, ctx->d_melout, d_mask,
-                          noise_state, d_is_noise, d_estimate, slot0, dtx_off);
+                          noise_state, d_is_noise, d_estimate, slot0, dtx_off, active, encoder_side);
 }
 
 // comfort noise of slots [slot0, slot0 + count) into ctx->d_cng_pcm on stream `st`: from `d_features` (log-mel by slot) or, when
@@ -513,12 +527,13 @@ int LaunchComfortNoise(lyra_b200_ctx* ctx, cudaStream_t st, const int* d_ids, in
 // 16 kHz rows to external-rate rows (the decoder's output side).  Each stream converts at its own rate (d_stream_rate; rows of a
 // stream below the context's rate use their first rate / 50 samples, decoder rows get zeros after them).  Whole hops from phase
 // 0 stay at phase 0 (the ratios are integers), so every row is exactly one hop.
-int LaunchCodecResample(lyra_b200_ctx* ctx, const Part& p, int dir, const int* d_ids, int n, const int16_t* in, int16_t* out) {
+int LaunchCodecResample(lyra_b200_ctx* ctx, const Part& p, int dir, const int* d_ids, int n, const int16_t* in, int16_t* out,
+                        const uint8_t* active) {
   const int ext = ctx->sample_rate / 50;
   const int in_stride = dir ? LYRA_B200_HOP : ext, out_stride = dir ? ext : LYRA_B200_HOP;
   return LAUNCH(kNoProf, ResampleKernel, dim3((unsigned)p.nslots), dim3(128), sizeof(float) * (size_t)(kResamplerTaps - 1 + in_stride), p.st,
                 ctx->d_blob, ctx->spec.resampler, dir ? 3 : 0, ctx->codec_rs_tag, d_ids, n, in, in_stride, in_stride, out, out_stride,
-                nullptr, ctx->d_codec_rs_delay[dir], ctx->d_codec_rs_pos[dir], p.slot0, ctx->d_stream_rate, ctx->sample_rate);
+                nullptr, ctx->d_codec_rs_delay[dir], ctx->d_codec_rs_pos[dir], p.slot0, ctx->d_stream_rate, ctx->sample_rate, active);
 }
 
 // The five fused codec calls; kEncode and kDecode are also GraphKey::kind
@@ -542,6 +557,7 @@ struct CodecCall {
   Io dev, host;
   int32_t* packet_bytes = nullptr;         // lyra_b200_encode_dtx: per row 0 for a DTX hop, else the packet's size
   const int* d_ids = nullptr;              // the ids on the device, for chains with kernels indexed by stream id
+  const uint8_t* active = nullptr;         // a twin's lyra_b200_set_active_mask buffer, by slot (nullptr: every stream runs)
 };
 
 // encode / encode_dtx.  PCM rows hold ctx->sample_rate / 50 samples (the external rate).  At 16 kHz the encoder reads the rows
@@ -552,6 +568,8 @@ struct CodecCall {
 // encoder (their streams' state does not advance) and get an empty packet (lyra/lyra_encoder.cc:131-141); flags[slot] = 1 marks
 // them.  The converter runs for those hops too: the reference resamples before its DTX branch (:118-135).  A stream whose DTX is
 // off (lyra_b200_set_stream_dtx) feeds no estimator and gets flag 0, so it is always encoded, as with enable_dtx = false.
+// A stream that sits out (c.active) is not converted; in encode_dtx its estimator writes flag 1, which the encoder nets and the
+// quantizer already skip, so only encode hands them the mask.
 int RunEncode(lyra_b200_ctx* ctx, const CodecCall& c) {
   const CodecCall::Io &d = c.dev, &h = c.host;
   const bool dtx = c.kind == kEncodeDtx;
@@ -561,18 +579,20 @@ int RunEncode(lyra_b200_ctx* ctx, const CodecCall& c) {
   const int16_t* in = h.pcm_in ? stage : d.pcm_in;
   const int16_t* pcm16 = rs ? ctx->d_pcm : in;
   const uint8_t* skip = dtx ? d.flags : nullptr;
+  const uint8_t* active = dtx ? nullptr : c.active;
   return ForEachPart(ctx, c.n, [&](const Part& p) {
     int rc = LYRA_B200_OK;
     if (h.pcm_in)
       CU(cudaMemcpyAsync(stage + (size_t)p.slot0 * hop, h.pcm_in + (size_t)p.slot0 * hop, sizeof(int16_t) * hop * (size_t)p.nslots,
                          cudaMemcpyHostToDevice, p.st));
-    if (rs && (rc = LaunchCodecResample(ctx, p, 0, c.d_ids, c.n, in, ctx->d_pcm))) return rc;
+    if (rs && (rc = LaunchCodecResample(ctx, p, 0, c.d_ids, c.n, in, ctx->d_pcm, c.active))) return rc;
     if (dtx) {
-      if ((rc = LaunchNoiseUpdate(ctx, p.st, c.d_ids, p.slot0, p.nslots, c.n, pcm16, nullptr, d.flags, nullptr, true))) return rc;
+      if ((rc = LaunchNoiseUpdate(ctx, p.st, c.d_ids, p.slot0, p.nslots, c.n, pcm16, nullptr, d.flags, nullptr, true, c.active))) return rc;
       if (h.flags) CU(cudaMemcpyAsync(h.flags + p.slot0, d.flags + p.slot0, (size_t)p.nslots, cudaMemcpyDeviceToHost, p.st));
     }
-    if ((rc = LaunchEncoderNets(ctx, p, skip, pcm16, ctx->d_features))) return rc;
-    if ((rc = LaunchQuantize(ctx, p, ctx->d_features, c.num_bits, d.packets_out, nullptr, skip, StreamWord(ctx, kWordEncBits), c.d_ids)))
+    if ((rc = LaunchEncoderNets(ctx, p, skip, pcm16, ctx->d_features, active))) return rc;
+    if ((rc = LaunchQuantize(ctx, p, ctx->d_features, c.num_bits, d.packets_out, nullptr, skip, StreamWord(ctx, kWordEncBits), c.d_ids,
+                             active)))
       return rc;
     if (h.packets_out)
       CU(cudaMemcpyAsync(h.packets_out + (size_t)p.slot0 * pb, d.packets_out + (size_t)p.slot0 * pb, pb * (size_t)p.nslots, cudaMemcpyDeviceToHost, p.st));
@@ -584,7 +604,9 @@ int RunEncode(lyra_b200_ctx* ctx, const CodecCall& c) {
 // (received streams only), as LyraDecoder::DecodeSamplesInternal does (lyra/lyra_decoder.cc:306-311).  PCM rows hold
 // ctx->sample_rate / 50 samples.  At another rate than 16 kHz the decoder writes the 16 kHz scratch ctx->d_pcm, the estimator is
 // fed from it (it stays at 16 kHz, lyra/lyra_decoder.cc:122-132), and one up-sampling launch per part writes the external-rate
-// rows (to ctx->d_rs_out for a host-buffer call).
+// rows (to ctx->d_rs_out for a host-buffer call).  A stream that sits out (c.active) reads no packet, advances no state and
+// gets a zero row (written by the RVQ decode at 16 kHz, which the decoder nets then skip, or by the converter); its noise flag
+// reports the estimator as it is.
 int RunDecode(lyra_b200_ctx* ctx, const CodecCall& c) {
   const CodecCall::Io &d = c.dev, &h = c.host;
   const size_t pb = (size_t)PacketBytes(c.num_bits), hop = (size_t)ctx->sample_rate / 50;
@@ -597,13 +619,16 @@ int RunDecode(lyra_b200_ctx* ctx, const CodecCall& c) {
       CU(cudaMemcpyAsync(ctx->d_packets + (size_t)p.slot0 * pb, h.packets_in + (size_t)p.slot0 * pb, pb * (size_t)p.nslots, cudaMemcpyHostToDevice, p.st));
     if (h.received)
       CU(cudaMemcpyAsync(ctx->d_received + p.slot0, h.received + p.slot0, (size_t)p.nslots, cudaMemcpyHostToDevice, p.st));
-    if ((rc = LaunchDequantize(ctx, p, d.packets_in, d.received, c.num_bits, ctx->d_features, StreamWord(ctx, kWordDecBits), c.d_ids))) return rc;
-    if ((rc = LaunchDecoderNets(ctx, p, nullptr, ctx->d_features, pcm16))) return rc;
+    if ((rc = LaunchDequantize(ctx, p, d.packets_in, d.received, c.num_bits, ctx->d_features, StreamWord(ctx, kWordDecBits), c.d_ids,
+                               c.active, rs ? nullptr : out)))
+      return rc;
+    if ((rc = LaunchDecoderNets(ctx, p, nullptr, ctx->d_features, pcm16, c.active))) return rc;
     if (c.kind == kDecodeTrackNoise) {
-      if ((rc = LaunchNoiseUpdate(ctx, p.st, c.d_ids, p.slot0, p.nslots, c.n, pcm16, d.received, d.flags, nullptr))) return rc;
+      if ((rc = LaunchNoiseUpdate(ctx, p.st, c.d_ids, p.slot0, p.nslots, c.n, pcm16, d.received, d.flags, nullptr, false, c.active)))
+        return rc;
       if (h.flags) CU(cudaMemcpyAsync(h.flags + p.slot0, d.flags + p.slot0, (size_t)p.nslots, cudaMemcpyDeviceToHost, p.st));
     }
-    if (rs && (rc = LaunchCodecResample(ctx, p, 1, c.d_ids, c.n, pcm16, out))) return rc;
+    if (rs && (rc = LaunchCodecResample(ctx, p, 1, c.d_ids, c.n, pcm16, out, c.active))) return rc;
     if (h.pcm_out)
       CU(cudaMemcpyAsync(h.pcm_out + (size_t)p.slot0 * hop, out + (size_t)p.slot0 * hop, sizeof(int16_t) * hop * (size_t)p.nslots,
                          cudaMemcpyDeviceToHost, p.st));
@@ -616,6 +641,8 @@ int RunDecode(lyra_b200_ctx* ctx, const CodecCall& c) {
 // model audio -> comfort noise from the current noise estimates for the streams that need it -> cross-fade -> noise-estimator
 // update of the streams that decoded a received packet.  One whole hop per stream and call.  PCM rows and the conversion to the
 // external rate as in RunDecode: the cross-fade writes the 16 kHz scratch, one up-sampling launch per part writes the rows.
+// A stream that sits out (c.active) gets plan kPlanSatOut from PlcPlanKernel: the plan's skip and feed bytes keep it out of the
+// decoder nets and the noise update, the comfort-noise generator skips it and the cross-fade writes zeros.
 int RunDecodePlc(lyra_b200_ctx* ctx, const CodecCall& c) {
   const CodecCall::Io &d = c.dev, &h = c.host;
   const size_t pb = (size_t)PacketBytes(c.num_bits), hop = (size_t)ctx->sample_rate / 50;
@@ -624,13 +651,16 @@ int RunDecodePlc(lyra_b200_ctx* ctx, const CodecCall& c) {
   int16_t* pcm16 = rs ? ctx->d_pcm : out;
   if (h.received) CU(cudaMemcpyAsync(ctx->d_received, h.received, (size_t)c.n, cudaMemcpyHostToDevice, ctx->stream));
   if (int rc = LAUNCH(kNoProf, PlcPlanKernel, dim3((unsigned)((c.n + 255) / 256)), dim3(256), (size_t)0, ctx->stream,
-                      c.d_ids, c.n, d.received, ctx->d_plc, ctx->d_plan, ctx->d_fade0, ctx->d_dir, ctx->d_skip, ctx->d_feed, d.flags))
+                      c.d_ids, c.n, d.received, ctx->d_plc, ctx->d_plan, ctx->d_fade0, ctx->d_dir, ctx->d_skip, ctx->d_feed, d.flags,
+                      c.active))
     return rc;
   return ForEachPart(ctx, c.n, [&](const Part& p) {
     int rc = LYRA_B200_OK;
     if (h.packets_in)
       CU(cudaMemcpyAsync(ctx->d_packets + (size_t)p.slot0 * pb, h.packets_in + (size_t)p.slot0 * pb, pb * (size_t)p.nslots, cudaMemcpyHostToDevice, p.st));
-    if ((rc = LaunchDequantize(ctx, p, d.packets_in, d.received, c.num_bits, ctx->d_features, StreamWord(ctx, kWordDecBits), c.d_ids))) return rc;
+    if ((rc = LaunchDequantize(ctx, p, d.packets_in, d.received, c.num_bits, ctx->d_features, StreamWord(ctx, kWordDecBits), c.d_ids,
+                               c.active)))
+      return rc;
     if ((rc = LaunchDecoderNets(ctx, p, ctx->d_skip, ctx->d_features, ctx->d_model_pcm))) return rc;
     if ((rc = LaunchComfortNoise(ctx, p.st, c.d_ids, p.slot0, p.nslots, c.n, nullptr, ctx->d_plan))) return rc;
     if ((rc = LAUNCH(kNoProf, PlcMixKernel, dim3((unsigned)p.nslots), dim3(320), (size_t)0, p.st,
@@ -638,7 +668,7 @@ int RunDecodePlc(lyra_b200_ctx* ctx, const CodecCall& c) {
                      ctx->d_model_pcm + (size_t)p.slot0 * 320, ctx->d_cng_pcm + (size_t)p.slot0 * 320, pcm16 + (size_t)p.slot0 * 320)))
       return rc;
     if ((rc = LaunchNoiseUpdate(ctx, p.st, c.d_ids, p.slot0, p.nslots, c.n, ctx->d_model_pcm, ctx->d_feed, nullptr, nullptr))) return rc;
-    if (rs && (rc = LaunchCodecResample(ctx, p, 1, c.d_ids, c.n, pcm16, out))) return rc;
+    if (rs && (rc = LaunchCodecResample(ctx, p, 1, c.d_ids, c.n, pcm16, out, c.active))) return rc;
     if (h.pcm_out)
       CU(cudaMemcpyAsync(h.pcm_out + (size_t)p.slot0 * hop, out + (size_t)p.slot0 * hop, sizeof(int16_t) * hop * (size_t)p.nslots,
                          cudaMemcpyDeviceToHost, p.st));
@@ -829,6 +859,8 @@ int RunCodecCall(lyra_b200_ctx* ctx, CodecCall c) {
     c.dev.pcm_in = c.dev.pcm_out = ctx->d_pcm;
     c.dev.packets_in = c.dev.packets_out = ctx->d_packets;
     c.dev.received = c.host.received ? ctx->d_received : nullptr;
+  } else {
+    c.active = ctx->d_active;                       // only the *_device twins read the mask: a host call's ids say who runs
   }
   if (!c.dev.flags) c.dev.flags = c.kind == kDecodePlc ? ctx->d_is_cn : ctx->d_is_noise;
   std::vector<uint8_t> dtx_flags;
@@ -1405,6 +1437,12 @@ int lyra_b200_stream_dtx(lyra_b200_ctx* ctx, const int32_t* stream_ids, int n, i
   return LYRA_B200_OK;
 }
 
+int lyra_b200_set_active_mask(lyra_b200_ctx* ctx, const uint8_t* d_active) {
+  if (!ctx) return LYRA_B200_EINVAL;
+  ctx->d_active = d_active;          // read by the kernels of later *_device codec calls, in stream order
+  return LYRA_B200_OK;
+}
+
 int lyra_b200_synchronize(lyra_b200_ctx* ctx) {
   if (!ctx) return LYRA_B200_EINVAL;
   ENTER(0);
@@ -1693,7 +1731,8 @@ int lyra_b200_resample(lyra_b200_ctx* ctx, int to_internal, const int32_t* ids, 
   const int dir = to_internal ? 0 : 1;
   if ((rc = LAUNCH(kNoProf, ResampleKernel, dim3((unsigned)n), dim3(128), sizeof(float) * (size_t)(kResamplerTaps - 1 + in_samples),
                    ctx->stream, ctx->d_blob, ctx->spec.resampler, pr, external_rate_hz, d_ids, n, ctx->d_rs_in, in_samples, in_samples,
-                   ctx->d_rs_out, out_stride, ctx->d_rs_counts, ctx->d_rs_delay[dir], ctx->d_rs_pos[dir], 0, nullptr, external_rate_hz)))
+                   ctx->d_rs_out, out_stride, ctx->d_rs_counts, ctx->d_rs_delay[dir], ctx->d_rs_pos[dir], 0, nullptr, external_rate_hz,
+                   nullptr)))
     return rc;
   CU(cudaMemcpyAsync(out, ctx->d_rs_out, sizeof(int16_t) * (size_t)out_stride * (size_t)n, cudaMemcpyDeviceToHost, ctx->stream));
   std::vector<int> counts((size_t)n);

@@ -102,6 +102,8 @@ struct TileIo {
   const int* slot_of_stream;   // [max_streams] position of the stream in this call's I/O arrays, -1 = not in this call
   const uint8_t* skip;         // optional, by slot: 1 = the stream sits this call out (its state does not advance): DTX noise
                                // hops on the encoder side, pure comfort-noise hops on the decoder side
+  const uint8_t* active;       // optional, by slot: 0 = the caller sits the stream out this call (lyra_b200_set_active_mask):
+                               // inactive like a skipped stream
 };
 
 // Per-tile metadata in shared memory: slot[S], active[S], n18[S] and n18[S] = the frame counter shared by all
@@ -114,7 +116,7 @@ __device__ __forceinline__ void LoadTileMeta(const TileIo& io, const int* n18_gl
     const int stream = tile * S + (int)threadIdx.x;
     const int sl = io.slot_of_stream[stream];
     slot[threadIdx.x] = sl;
-    active[threadIdx.x] = sl >= 0 && !(io.skip != nullptr && io.skip[sl]);
+    active[threadIdx.x] = sl >= 0 && !(io.active != nullptr && !io.active[sl]) && !(io.skip != nullptr && io.skip[sl]);
     n18[threadIdx.x] = n18_global[stream];
   }
   __syncthreads();

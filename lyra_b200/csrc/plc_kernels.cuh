@@ -19,15 +19,26 @@ constexpr int kPlcConcealSamples = 1280, kPlcFadeSamples = 640;
 //   then the decode step of lyra_decoder.cc:249-283 with num_samples_to_generate = 320.
 // plan[slot] bits: 1 = run the generative model, 2 = run the comfort-noise generator, 4 = the hop comes from a received packet
 // (feed the noise estimator); fade0[slot] = fade progress before the hop, dir[slot] = fade direction of the hop.
+// active (nullptr: every slot; lyra_b200_set_active_mask): a slot whose byte is 0 sits the tick out, as a LyraDecoder that is not
+// called: plan kPlanSatOut (no model, no comfort noise, no feed; PlcMixKernel writes zeros), its received byte is not read, its
+// state is not written and is_comfort_noise reports the state as it is.
+constexpr uint8_t kPlanSatOut = 8;
 __global__ void __launch_bounds__(256)
 PlcPlanKernel(const int* __restrict__ stream_ids, int n, const uint8_t* __restrict__ received, int* __restrict__ state,
               uint8_t* __restrict__ plan, int* __restrict__ fade0, int* __restrict__ dir_out, uint8_t* __restrict__ skip_model,
-              uint8_t* __restrict__ feed_mask, uint8_t* __restrict__ is_comfort_noise) {
+              uint8_t* __restrict__ feed_mask, uint8_t* __restrict__ is_comfort_noise, const uint8_t* __restrict__ active) {
   const int slot = (int)(blockIdx.x * blockDim.x + threadIdx.x);
   if (slot >= n) return;
   const int stream = stream_ids ? stream_ids[slot] : slot;
   int* st = state + (size_t)stream * 4;
   int cp = st[0], fp = st[1], dir = st[2];
+  if (active && !active[slot]) {
+    plan[slot] = kPlanSatOut;
+    skip_model[slot] = 1;
+    feed_mask[slot] = 0;
+    if (is_comfort_noise) is_comfort_noise[slot] = fp == kPlcFadeSamples ? 1 : 0;
+    return;
+  }
   const bool rec = received == nullptr || received[slot] != 0;
   if (rec && cp > 0) cp = 0;                                  // SetEncodedPacket :186-196 (nothing left of a fake hop at a hop boundary)
   const bool is_packet_received = rec && cp == 0;             // :249-251 (the model queue holds exactly this tick's packet)
@@ -140,6 +151,7 @@ PlcMixKernel(const uint8_t* __restrict__ blob, CngParams P, int n, const uint8_t
   if (slot >= n) return;
   const int pl = plan[slot];
   const size_t o = (size_t)slot * 320 + i;
+  if (pl == kPlanSatOut) { out[o] = 0; return; }
   if (!(pl & 2)) { out[o] = model_pcm[o]; return; }
   if (!(pl & 1)) { out[o] = cng_pcm[o]; return; }
   const float* fade = BlobPtr<float>(blob, P.fade);
@@ -173,11 +185,13 @@ NoiseReadKernel(const int* __restrict__ stream_ids, int n, const float* __restri
 // runs at its own rate r = StreamRate(rate_word, stream, rate) (`rate` = the context's): pair + RateIndex(r) - 1, r / 50 samples on
 // the external side, 320 on the 16 kHz side; a 16 kHz stream is copied through and its converter state is left alone.  Output rows
 // longer than the stream's hop (a decoder row of a stream below the context's rate) get zeros after it.
+// active (nullptr: every slot; lyra_b200_set_active_mask): a slot whose byte is 0 sits the call out - its input row and converter
+// state are neither read nor written; from 16 kHz (pair >= 3) its output row is written as zeros.
 __global__ void __launch_bounds__(128)
 ResampleKernel(const uint8_t* __restrict__ blob, ResamplerParams P, int pair, int tag, const int* __restrict__ stream_ids, int n,
                const int16_t* __restrict__ in, int in_stride, int n_in, int16_t* __restrict__ out, int out_stride,
                int* __restrict__ counts, int16_t* __restrict__ delay_state, int* __restrict__ pos_state, int slot_base,
-               const int* __restrict__ rate_word, int rate) {
+               const int* __restrict__ rate_word, int rate, const uint8_t* __restrict__ active) {
   unsigned char* smem = LYRA_DYN_SMEM();
   float* x = reinterpret_cast<float*>(smem);              // [34 + n_in]: delay line followed by the new samples
   const int slot = slot_base + (int)blockIdx.x;
@@ -187,6 +201,11 @@ ResampleKernel(const uint8_t* __restrict__ blob, ResamplerParams P, int pair, in
   const int tid = (int)threadIdx.x, NT = (int)blockDim.x;
   const int16_t* row = in + (size_t)slot * in_stride;
   int16_t* orow = out + (size_t)slot * out_stride;
+  if (active && !active[slot]) {
+    if (pair >= 3)
+      for (int j = tid; j < out_stride; j += NT) orow[j] = 0;
+    return;
+  }
   int n_out = out_stride;
   if (rate_word) {
     constexpr int H = 320;                                // one 16 kHz hop

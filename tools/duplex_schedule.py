@@ -6,7 +6,8 @@ Each group is an encoder-only and a decoder-only context of m streams, installed
 the slot's previous packets have been decoded, its decode waits for its packets through an event, and nothing synchronises
 the host.  The decode_plc workload runs decode_plc_device on the decoder contexts alone, over caller-supplied packets and
 received masks.  With `dtx` the encoders run encode_dtx_device into a flag buffer per slot, and the decoders take a DTX hop as a
-lost packet: received = 1 - flag, computed on the decoder's CUDA stream.
+lost packet: received = 1 - flag, computed on the decoder's CUDA stream.  With `mask` every context reads the active mask of
+hop i from pattern i % len(mask) (lyra_b200_set_active_mask): a stream that sits out a hop is neither encoded nor decoded.
 """
 import numpy as np
 import torch
@@ -23,12 +24,15 @@ def _row(t, g, m):
 
 class Schedule:
     def __init__(self, slots, groups, split, mode, bits=64, rate=16000, stream_rates=None, masks=None, keep_hops=0, stream_bits=None,
-                 dtx=None):
+                 dtx=None, mask=None, realign=0):
         """slots: NBUF host arrays of n rows, the input PCM (rate // 50 samples per row), or with `masks` (the decode_plc
         workload) the packets; masks: NBUF received masks of n entries.  stream_rates: the per-stream rates of every group's
         m streams; stream_bits: their per-stream bit counts (both roles, at most `bits`); dtx: their DTX settings (1 on, 0 off;
         None: no DTX, encode_device).  keep_hops: hop i < keep_hops writes its own output (and flag) buffer and keeps a copy of
-        its packets (and DTX flags), and the schedule runs at most keep_hops hops; with 0 every hop writes one shared output."""
+        its packets (and DTX flags), and the schedule runs at most keep_hops hops; with 0 every hop writes one shared output.
+        mask: active-mask patterns of n entries each (0 = the stream sits the hop out), hop i uses pattern i % len(mask) on both
+        contexts of every group; realign > 0: every `realign` hops both contexts align every stream with the first stream of its
+        tile (lyra_b200_align_streams), so tiles whose lanes sat out different hops are back on one hop counter."""
         n = len(slots[0])
         self.n, self.m, self.bits, self.keep_hops = n, n // groups, bits, keep_hops
         self.plc = masks is not None
@@ -44,6 +48,8 @@ class Schedule:
             self.dtx_flags = [torch.zeros((n,), dtype=torch.uint8, device="cuda") for _ in range(NBUF)]
             self.received = [torch.ones((n,), dtype=torch.bool, device="cuda") for _ in range(NBUF)]     # one byte, 0 or 1
             self.kept_flags = [torch.zeros_like(self.dtx_flags[0]) for _ in range(keep_hops)]
+        self.mask = None if mask is None else [dev(np.asarray(x, np.uint8)) for x in mask]
+        self.realign = realign
         outs = max(keep_hops, 1)
         self.out = [torch.full((n, rate // 50), 0x5A5A, dtype=torch.int16, device="cuda") for _ in range(outs)]
         self.flags = [torch.full((n,), 0xAA, dtype=torch.uint8, device="cuda") for _ in range(outs)] if self.plc else None
@@ -83,6 +89,15 @@ class Schedule:
             if i >= NBUF:
                 gx.wait_event(self.ev_free[g][b])
             rows = slice(g * m, (g + 1) * m)
+            if self.mask is not None:
+                p = _row(self.mask[i % len(self.mask)], g, m)
+                e_.set_active_mask(p)
+                d_.set_active_mask(p)
+                if self.realign and i and i % self.realign == 0:
+                    t = e_.tile_streams
+                    ids = np.array([k for k in range(m) if k % t], np.int32)
+                    for c in (e_, d_):
+                        c.align_streams(ids, ids // t * t)
             if self.dtx:
                 e_.encode_dtx_device(m, _row(self.pcm[b], g, m), bits, pk, _row(self.dtx_flags[b], g, m))
             else:

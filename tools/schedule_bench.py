@@ -21,7 +21,13 @@ run in one process so that clock and thermal drift hit them alike:
   dtx-mixed          dtx with DTX off for every other stream (lyra_b200_set_stream_dtx), so every tile mixes the two kinds;
   dtx-split          the same traffic split by kind: half the streams in encode_dtx_device pairs, half in encode_device pairs
                      (what a server without per-stream DTX runs);
-  dtx-off            dtx with DTX off for every stream, to compare with 16k.
+  dtx-off            dtx with DTX off for every stream, to compare with 16k;
+  mask-ones          16k with an all-ones active mask installed (lyra_b200_set_active_mask), to compare with 16k;
+  mask-tiles         16k with the tiles alternating hop by hop: the even tiles run on even hops, the odd tiles on odd hops (a
+                     server that ticks every 10 ms and staggers the 20 ms hop phase of its calls tile by tile);
+  mask-lanes         16k with a rotating quarter of the lanes of every tile sitting out (lanes 2k, 2k + 1 on hops i = k mod 4),
+                     every stream aligned with the first lane of its tile every 25 hops (lyra_b200_align_streams).
+Frames/s counts every stream's hops, also those it sits out; the mask configurations also report the active fraction.
 The dtx configurations also report the fraction of DTX hops over the timed runs.
 Prints one line per run, then every configuration's median, spread and ratio to the first configuration, the card's name,
 power limit and median SM clock over the timed runs, and a JSON line.  --profile-hops adds a torch.profiler pass per
@@ -29,7 +35,7 @@ configuration, separate from the timed runs: the mean device time per launch of 
 RvqDecodeKernel.
 
   python tools/schedule_bench.py [--configs 16k,48k,8k,mixed,split,bits-184,bits-mixed,bits-split,mixed-counters,aligned-counters,
-                                            dtx,dtx-mixed,dtx-split,dtx-off]
+                                            dtx,dtx-mixed,dtx-split,dtx-off,mask-ones,mask-tiles,mask-lanes]
                                  [--streams 4096]
                                  [--hops 200] [--runs 5]
 """
@@ -50,8 +56,14 @@ import duplex_schedule as ds  # noqa: E402
 RATES = (8000, 16000, 32000, 48000)
 BIT_RATES = (64, 120, 184)
 CONFIGS = ("16k", "8k", "32k", "48k", "mixed", "split", "bits-184", "bits-mixed", "bits-split", "mixed-counters", "aligned-counters",
-           "dtx", "dtx-mixed", "dtx-split", "dtx-off")
+           "dtx", "dtx-mixed", "dtx-split", "dtx-off", "mask-ones", "mask-tiles", "mask-lanes")
 PROFILED = ("ResampleKernel", "RvqEncodeKernel", "RvqDecodeKernel")
+# active-mask patterns of the mask-* configurations (rows of all groups, 8-stream tiles), applied hop by hop in turn
+MASKS = {
+    "mask-ones": lambda n: [np.ones(n, np.uint8)],
+    "mask-tiles": lambda n: [((np.arange(n) // 8) % 2 == h).astype(np.uint8) for h in range(2)],
+    "mask-lanes": lambda n: [((np.arange(n) % 8) // 2 != k).astype(np.uint8) for k in range(4)],
+}
 
 
 def power_limit():
@@ -75,16 +87,18 @@ def speech_slots(streams):
 
 def make(name, args):
     """The schedules of one configuration."""
-    def sched(n, groups, rate=16000, stream_rates=None, bits=None, stream_bits=None, dtx=None, speech=None):
+    def sched(n, groups, rate=16000, stream_rates=None, bits=None, stream_bits=None, dtx=None, speech=None, mask=None, realign=0):
         if speech is None:
             rng = np.random.default_rng(1234)
             pcm = [rng.integers(-8192, 8192, size=(n, rate // 50), dtype=np.int16) for _ in range(ds.NBUF)]
         else:
             pcm = speech_slots(speech)
         return ds.Schedule(pcm, groups, args.split, args.decoder_mode, bits or args.bits, rate=rate, stream_rates=stream_rates,
-                           stream_bits=stream_bits, dtx=dtx)
+                           stream_bits=stream_bits, dtx=dtx, mask=mask, realign=realign)
 
     n, g = args.streams, args.groups
+    if name.startswith("mask-"):
+        return [sched(n, g, mask=MASKS[name](n), realign=25 if name == "mask-lanes" else 0)]
     if name in ("dtx", "dtx-mixed", "dtx-off"):
         m = n // g
         dtx = {"dtx": np.ones(m, np.int32), "dtx-mixed": (np.arange(m) % 2 == 0).astype(np.int32), "dtx-off": np.zeros(m, np.int32)}[name]
@@ -183,6 +197,7 @@ def main():
         "bits": args.bits, "decoder_mode": args.decoder_mode, "split": args.split, "groups": args.groups, "hops_per_run": args.hops,
         "frames_per_s": fps, "median_frames_per_s": med, "spread": {k: [min(v) / med[k], max(v) / med[k]] for k, v in fps.items()},
         "ratio_to_" + base: {k: v / med[base] for k, v in med.items()}, "kernels": kernel, "dtx_hop_fraction": dtx_frac,
+        "active_fraction": {k: float(np.mean([p.mean() for p in MASKS[k](args.streams)])) for k in names if k in MASKS},
     }
     for k in names:
         print("%-14s: median %.3f M frames/s (runs %.3f-%.3f), %.3f x %s%s" % (
