@@ -12,6 +12,7 @@
 #define LYRA_SET_MAX_SMEM(kernel, bytes) (0)
 #define LYRA_DEVICE_CODE 1
 #define LYRA_TRAP() std::abort()
+#define __grid_constant__
 #else
 #include <cuda_runtime.h>
 #define LYRA_DYN_SMEM() (lyra_dyn_smem_raw)

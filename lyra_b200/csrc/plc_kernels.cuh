@@ -19,20 +19,19 @@ constexpr int kPlcConcealSamples = 1280, kPlcFadeSamples = 640;
 //   then the decode step of lyra_decoder.cc:249-283 with num_samples_to_generate = 320.
 // plan[slot] bits: 1 = run the generative model, 2 = run the comfort-noise generator, 4 = the hop comes from a received packet
 // (feed the noise estimator); fade0[slot] = fade progress before the hop, dir[slot] = fade direction of the hop.
-// active (nullptr: every slot; lyra_b200_set_active_mask): a slot whose byte is 0 sits the tick out, as a LyraDecoder that is not
-// called: plan kPlanSatOut (no model, no comfort noise, no feed; PlcMixKernel writes zeros), its received byte is not read, its
-// state is not written and is_comfort_noise reports the state as it is.
+// A slot that sits out does so as a LyraDecoder that is not called: plan kPlanSatOut (no model, no comfort noise, no feed;
+// PlcMixKernel writes zeros), its received byte is not read, its state is not written and is_comfort_noise reports the state as
+// it is.
 constexpr uint8_t kPlanSatOut = 8;
 __global__ void __launch_bounds__(256)
-PlcPlanKernel(const int* __restrict__ stream_ids, int n, const uint8_t* __restrict__ received, int* __restrict__ state,
+PlcPlanKernel(const __grid_constant__ RowIo io, const uint8_t* __restrict__ received, int* __restrict__ state,
               uint8_t* __restrict__ plan, int* __restrict__ fade0, int* __restrict__ dir_out, uint8_t* __restrict__ skip_model,
-              uint8_t* __restrict__ feed_mask, uint8_t* __restrict__ is_comfort_noise, const uint8_t* __restrict__ active) {
-  const int slot = (int)(blockIdx.x * blockDim.x + threadIdx.x);
-  if (slot >= n) return;
-  const int stream = stream_ids ? stream_ids[slot] : slot;
-  int* st = state + (size_t)stream * 4;
+              uint8_t* __restrict__ feed_mask, uint8_t* __restrict__ is_comfort_noise) {
+  const int row = (int)(blockIdx.x * blockDim.x + threadIdx.x), slot = io.slot0 + row;
+  if (row >= io.slots) return;
+  int* st = state + (size_t)io.Stream(slot) * 4;
   int cp = st[0], fp = st[1], dir = st[2];
-  if (active && !active[slot]) {
+  if (io.SatOut(slot)) {
     plan[slot] = kPlanSatOut;
     skip_model[slot] = 1;
     feed_mask[slot] = 0;
@@ -68,27 +67,26 @@ __device__ __forceinline__ uint32_t CngPhaseIndex(unsigned long long seed, unsig
   return (uint32_t)(x >> 54);
 }
 
-// One block of 128 threads per stream.  features: [n][160] conditioning log-mel vectors (by slot), or nullptr = the stream's
+// One block of 128 threads per stream.  features: [slots][160] conditioning log-mel vectors (by slot), or nullptr = the stream's
 // current noise estimate (the first 160 floats of its noise-estimator state, LyraDecoder::RunComfortNoiseGenerator,
 // lyra/lyra_decoder.cc:328-340).  plan: nullptr = every slot runs; otherwise only slots with bit 2.
 // work: [max_streams][1024] f64 overlap-add buffers; hops: [max_streams][2] {hop counter, key offset}: the phases of stream s are
 // drawn from key seed + s + offset (offset 0 unless the stream's state was moved here by lyra_b200_import_streams / _copy_streams).
 constexpr int kCngThreads = 128;
 __global__ void __launch_bounds__(kCngThreads)
-ComfortNoiseKernel(const uint8_t* __restrict__ blob, CngParams P, const int* __restrict__ stream_ids, int n,
-                   const float* __restrict__ features, const float* __restrict__ noise_state, int noise_units,
-                   const uint8_t* __restrict__ plan, double* __restrict__ work, unsigned long long* __restrict__ hops,
-                   unsigned long long seed, int16_t* __restrict__ out, int slot_base) {
+ComfortNoiseKernel(const uint8_t* __restrict__ blob, CngParams P, const __grid_constant__ RowIo io, const float* __restrict__ features,
+                   const float* __restrict__ noise_state, int noise_units, const uint8_t* __restrict__ plan, double* __restrict__ work,
+                   unsigned long long* __restrict__ hops, unsigned long long seed, int16_t* __restrict__ out) {
   unsigned char* smem = LYRA_DYN_SMEM();
   double* re = reinterpret_cast<double*>(smem);
   double* im = re + kLogMelFftPadded;
   double* xr0 = im + kLogMelFftPadded;           // spectrum in natural order: real | imag, padded like the FFT buffers
   double* xi0 = xr0 + kLogMelFftPadded;
   double* mel = xi0 + kLogMelFftPadded;          // [160]
-  const int slot = slot_base + (int)blockIdx.x;
-  if (slot >= n) return;
+  if ((int)blockIdx.x >= io.slots) return;
+  const int slot = io.slot0 + (int)blockIdx.x;
   if (plan && !(plan[slot] & 2)) return;
-  const int stream = stream_ids ? stream_ids[slot] : slot;
+  const int stream = io.Stream(slot);
   const int tid = (int)threadIdx.x;
   constexpr int NT = kCngThreads, N = kLogMelFft;
   const double* wts = BlobPtr<double>(blob, P.weights);
@@ -144,11 +142,11 @@ ComfortNoiseKernel(const uint8_t* __restrict__ blob, CngParams P, const int* __r
 
 // out = model hop, comfort-noise hop, or their raised-cosine cross-fade (lyra_decoder.cc:342-373); 320 threads per slot
 __global__ void __launch_bounds__(320)
-PlcMixKernel(const uint8_t* __restrict__ blob, CngParams P, int n, const uint8_t* __restrict__ plan, const int* __restrict__ fade0,
-             const int* __restrict__ dir, const int16_t* __restrict__ model_pcm, const int16_t* __restrict__ cng_pcm,
-             int16_t* __restrict__ out) {
-  const int slot = (int)blockIdx.x, i = (int)threadIdx.x;
-  if (slot >= n) return;
+PlcMixKernel(const uint8_t* __restrict__ blob, CngParams P, const __grid_constant__ RowIo io, const uint8_t* __restrict__ plan,
+             const int* __restrict__ fade0, const int* __restrict__ dir, const int16_t* __restrict__ model_pcm,
+             const int16_t* __restrict__ cng_pcm, int16_t* __restrict__ out) {
+  if ((int)blockIdx.x >= io.slots) return;
+  const int slot = io.slot0 + (int)blockIdx.x, i = (int)threadIdx.x;
   const int pl = plan[slot];
   const size_t o = (size_t)slot * 320 + i;
   if (pl == kPlanSatOut) { out[o] = 0; return; }
@@ -162,12 +160,11 @@ PlcMixKernel(const uint8_t* __restrict__ blob, CngParams P, int n, const uint8_t
 
 // read-only view of the noise estimators (NoiseEstimator::noise_estimate / is_noise, lyra/noise_estimator.h:55-62)
 __global__ void __launch_bounds__(192)
-NoiseReadKernel(const int* __restrict__ stream_ids, int n, const float* __restrict__ state, int nf, float* __restrict__ estimate_out,
+NoiseReadKernel(const __grid_constant__ RowIo io, const float* __restrict__ state, int nf, float* __restrict__ estimate_out,
                 uint8_t* __restrict__ is_noise_out) {
-  const int slot = (int)blockIdx.x, i = (int)threadIdx.x;
-  if (slot >= n) return;
-  const int stream = stream_ids ? stream_ids[slot] : slot;
-  const float* st = state + (size_t)stream * NoiseStateUnits(nf);
+  if ((int)blockIdx.x >= io.slots) return;
+  const int slot = io.slot0 + (int)blockIdx.x, i = (int)threadIdx.x;
+  const float* st = state + (size_t)io.Stream(slot) * NoiseStateUnits(nf);
   if (estimate_out && i < nf) estimate_out[(size_t)slot * nf + i] = st[i];
   if (is_noise_out && i == 0) is_noise_out[slot] = reinterpret_cast<const int*>(st + 5 * nf)[2] ? 0 : 1;
 }
@@ -178,38 +175,39 @@ NoiseReadKernel(const int* __restrict__ stream_ids, int n, const float* __restri
 // to the next input sample, in units of 1 / den input samples; tag = the configuration the state belongs to (lyra_b200_resample:
 // the external rate; the codec path: the generation of the context's rate setting).  A call with another tag starts from the
 // fully-primed state, like a fresh Resampler; 0 (what lyra_b200_reset writes) never matches.  counts[slot] (may be nullptr) =
-// outputs produced (they differ by at most one between streams when down-sampling from different phases).  I/O arrays are indexed
-// by slot: block b handles slot slot_base + b of a call of n slots; in rows are `in_stride` and out rows `out_stride` samples apart.
-// rate_word == nullptr (lyra_b200_resample): every stream converts n_in samples with `pair`, at most out_stride outputs.
-// rate_word != nullptr (the fused codec calls, one whole hop per row): pair is 0 (to 16 kHz) or 3 (from 16 kHz) and each stream
-// runs at its own rate r = StreamRate(rate_word, stream, rate) (`rate` = the context's): pair + RateIndex(r) - 1, r / 50 samples on
-// the external side, 320 on the 16 kHz side; a 16 kHz stream is copied through and its converter state is left alone.  Output rows
-// longer than the stream's hop (a decoder row of a stream below the context's rate) get zeros after it.
-// active (nullptr: every slot; lyra_b200_set_active_mask): a slot whose byte is 0 sits the call out - its input row and converter
-// state are neither read nor written; from 16 kHz (pair >= 3) its output row is written as zeros.
+// outputs produced (they differ by at most one between streams when down-sampling from different phases).  In rows are
+// `in_stride` and out rows `out_stride` samples apart.
+// words.rate == nullptr (lyra_b200_resample): every stream converts n_in samples with `pair`, at most out_stride outputs.
+// words.rate != nullptr (the fused codec calls, one whole hop per row): pair is 0 (to 16 kHz) or 3 (from 16 kHz) and each stream
+// runs at its own rate r: pair + RateIndex(r) - 1, r / 50 samples on the external side, 320 on the 16 kHz side; a 16 kHz stream is
+// copied through and its converter state is left alone.  Output rows longer than the stream's hop (a decoder row of a stream
+// below the context's rate) get zeros after it.
+// A slot that sits out has its input row and converter state neither read nor written; from 16 kHz (pair >= 3) its output row is
+// written as zeros.
 __global__ void __launch_bounds__(128)
-ResampleKernel(const uint8_t* __restrict__ blob, ResamplerParams P, int pair, int tag, const int* __restrict__ stream_ids, int n,
-               const int16_t* __restrict__ in, int in_stride, int n_in, int16_t* __restrict__ out, int out_stride,
-               int* __restrict__ counts, int16_t* __restrict__ delay_state, int* __restrict__ pos_state, int slot_base,
-               const int* __restrict__ rate_word, int rate, const uint8_t* __restrict__ active) {
+ResampleKernel(const uint8_t* __restrict__ blob, ResamplerParams P, int pair, int tag, const __grid_constant__ RowIo io,
+               const __grid_constant__ StreamWords words, const int16_t* __restrict__ in, int in_stride, int n_in,
+               int16_t* __restrict__ out, int out_stride, int* __restrict__ counts, int16_t* __restrict__ delay_state,
+               int* __restrict__ pos_state) {
   unsigned char* smem = LYRA_DYN_SMEM();
   float* x = reinterpret_cast<float*>(smem);              // [34 + n_in]: delay line followed by the new samples
-  const int slot = slot_base + (int)blockIdx.x;
-  if (slot >= n) return;
-  const int stream = stream_ids ? stream_ids[slot] : slot;
+  if ((int)blockIdx.x >= io.slots) return;
+  const int slot = io.slot0 + (int)blockIdx.x;
+  const int stream = io.Stream(slot);
   constexpr int T = kResamplerTaps;
   const int tid = (int)threadIdx.x, NT = (int)blockDim.x;
   const int16_t* row = in + (size_t)slot * in_stride;
   int16_t* orow = out + (size_t)slot * out_stride;
-  if (active && !active[slot]) {
+  if (io.SatOut(slot)) {
     if (pair >= 3)
       for (int j = tid; j < out_stride; j += NT) orow[j] = 0;
     return;
   }
   int n_out = out_stride;
-  if (rate_word) {
+  const bool codec = words.rate != nullptr;
+  if (codec) {
     constexpr int H = 320;                                // one 16 kHz hop
-    const int r = StreamRate(rate_word, stream, rate), k = RateIndex(r);
+    const int r = words.Rate(stream), k = RateIndex(r);
     if (k == 0) {                                         // 16 kHz: no conversion
       for (int j = tid; j < out_stride; j += NT) orow[j] = j < H ? row[j] : (int16_t)0;
       return;
@@ -229,7 +227,7 @@ ResampleKernel(const uint8_t* __restrict__ blob, ResamplerParams P, int pair, in
   const float* coeffs = BlobPtr<float>(blob, P.coeffs[pair]);
   const int total = n_in * den;
   const int count = a0 < total ? (total - a0 + num - 1) / num : 0;
-  if (rate_word)
+  if (codec)
     for (int j = (count < n_out ? count : n_out) + tid; j < out_stride; j += NT) orow[j] = 0;
   for (int j = tid; j < count && j < n_out; j += NT) {
     const int a = a0 + j * num, i = a / den, ph = a % den;
