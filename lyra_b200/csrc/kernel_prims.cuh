@@ -384,7 +384,11 @@ __host__ __device__ constexpr int PadLd(int x) {
 // ------------------------------------------------------------------------------------------------
 // fp32 tap-GEMM on the tensor cores in split precision ("3xTF32"); decoder tensor-core mode only.
 //   x = hi + lo with hi = the top 19 bits of x (what a TF32 operand keeps) and lo = x - hi (exact in fp32);
-//   a*b ~= a_lo*b_hi + a_hi*b_lo + a_hi*b_hi, accumulated in fp32 by mma.sync m16n8k8 (small terms first).
+//   a*b ~= a_lo*b_hi + a_hi*b_lo + a_hi*b_hi, accumulated in fp32 by mma.sync m16n8k8.  The two small terms have an
+//   accumulator of their own, added to the a_hi*b_hi one with one round-to-nearest add at the end: the tensor cores truncate
+//   while they accumulate, so every MMA folded into the large running sum adds a truncation error of that sum's size (with
+//   the small terms in the same accumulator, three per k-step instead of one: on an H100 max 5 LSB and 3.7 % of the decoded
+//   samples off the exact mode, against 4 LSB and 2.4 % with this and the same split in DecoderKernelDW).
 //   The dropped a_lo*b_lo term and the TF32 truncation of lo are both below 2^-21 relative, i.e. the result
 //   carries fp32-level accuracy but NOT the oracle's exact fmaf-chain rounding: outputs of this mode are
 //   compared with a tolerance (DESIGN.md, tests/test_gpu_parity.py), never bit-for-bit.
@@ -411,7 +415,7 @@ __device__ __forceinline__ void GemmTf32Mma(const float* A, int ldA, int rowA0, 
   const int M = T_out * S, MT = (M + 15) / 16, MTW = (MT + WTM - 1) / WTM, NTILES = N / 8, NWT = MTW * (NTILES / WTN);
   const int KS = ntaps * CinG / 8, CoutG = N / groups;
   const size_t ks_stride = (size_t)NTILES * 32;
-  float acc[WTM][WTN][4];
+  float acc[WTM][WTN][4], accs[WTM][WTN][4];          // a_hi*b_hi terms | a_lo*b_hi + a_hi*b_lo terms
   int tr[WTM][2], sr[WTM][2];
   bool vr[WTM][2];
   int nt0 = 0;
@@ -434,7 +438,9 @@ __device__ __forceinline__ void GemmTf32Mma(const float* A, int ldA, int rowA0, 
 #pragma unroll
     for (int i = 0; i < WTM; ++i)
 #pragma unroll
-      for (int j = 0; j < WTN; ++j) { acc[i][j][0] = 0.0f; acc[i][j][1] = 0.0f; acc[i][j][2] = 0.0f; acc[i][j][3] = 0.0f; }
+      for (int j = 0; j < WTN; ++j)
+#pragma unroll
+        for (int e = 0; e < 4; ++e) acc[i][j][e] = accs[i][j][e] = 0.0f;
     const float2* wp = Wf + (size_t)nt0 * 32 + lane;
     float2 bf[PD][WTN];
 #pragma unroll
@@ -465,8 +471,8 @@ __device__ __forceinline__ void GemmTf32Mma(const float* A, int ldA, int rowA0, 
             SplitTf32(bf[p][j].y, bhi[1], blo[1]);
 #pragma unroll
             for (int i = 0; i < WTM; ++i) {
-              lyra_mma_tf32_16x8x8(acc[i][j], alo[i], bhi);
-              lyra_mma_tf32_16x8x8(acc[i][j], ahi[i], blo);
+              lyra_mma_tf32_16x8x8(accs[i][j], alo[i], bhi);
+              lyra_mma_tf32_16x8x8(accs[i][j], ahi[i], blo);
               lyra_mma_tf32_16x8x8(acc[i][j], ahi[i], bhi);
             }
           }
@@ -477,6 +483,12 @@ __device__ __forceinline__ void GemmTf32Mma(const float* A, int ldA, int rowA0, 
         }
       }
     }
+#pragma unroll
+    for (int i = 0; i < WTM; ++i)
+#pragma unroll
+      for (int j = 0; j < WTN; ++j)
+#pragma unroll
+        for (int e = 0; e < 4; ++e) acc[i][j][e] = __fadd_rn(acc[i][j][e], accs[i][j][e]);
   };
   auto epilogue = [&]() {
 #pragma unroll

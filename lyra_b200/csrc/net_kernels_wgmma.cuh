@@ -265,9 +265,11 @@ DecoderKernelDW(const uint8_t* __restrict__ blob, DecoderParams P, TileIo io, co
     if (tid == 0) { lyra_bulk_s2g(st + (size_t)DecStateD::kUp2 * S, ov, 64u * 5 * S * 4); lyra_bulk_commit(); }
   }
 
-  // One 64 x 64 GEMM of the tile on the next two weight chunks: acc = A * W, A as split fragments (hi, lo) per k-step
+  // One 64 x 64 GEMM of the tile on the next two weight chunks: acc = A * W, A as split fragments (hi, lo) per k-step.  The small
+  // terms accumulate apart from a_hi * b_hi and join it with one round-to-nearest add (see GemmTf32Mma)
   auto gemm = [&](const uint32_t (&ah)[8][4], const uint32_t (&al)[8][4], float (&acc)[32]) {
     const uint32_t lboW = 8u * 128u;
+    float accs[32];
 #pragma unroll
     for (int kc = 0; kc < 2; ++kc) {
       const unsigned char* wst = wait_chunk();
@@ -277,14 +279,16 @@ DecoderKernelDW(const uint8_t* __restrict__ blob, DecoderParams P, TileIo io, co
         const int ks = kc * 4 + k4;
         const uint64_t bh = lyra_wgmma_desc(wst + (size_t)k4 * 2 * lboW, lboW, 128);
         const uint64_t bl = lyra_wgmma_desc(wst + kDuChunkBytes / 2 + (size_t)k4 * 2 * lboW, lboW, 128);
-        lyra_wgmma_m64n64_tf32_rs(acc, al[ks], bh, ks > 0);
-        lyra_wgmma_m64n64_tf32_rs(acc, ah[ks], bl, true);
-        lyra_wgmma_m64n64_tf32_rs(acc, ah[ks], bh, true);
+        lyra_wgmma_m64n64_tf32_rs(accs, al[ks], bh, ks > 0);
+        lyra_wgmma_m64n64_tf32_rs(accs, ah[ks], bl, true);
+        lyra_wgmma_m64n64_tf32_rs(acc, ah[ks], bh, ks > 0);
       }
       lyra_wgmma_commit();
       lyra_wgmma_wait<0>();
       release_chunk();
     }
+#pragma unroll
+    for (int i = 0; i < 32; ++i) acc[i] = __fadd_rn(acc[i], accs[i]);
   };
   // accumulator element i of the thread: GEMM row m0 (+ 8 for odd pairs), column (channel) 8 (i / 4) + 2 tq + i % 2
   auto acc_row = [&](int i) { return m0 + 8 * ((i >> 1) & 1); };
