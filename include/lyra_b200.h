@@ -307,6 +307,33 @@ int lyra_b200_decode_plc_device(lyra_b200_ctx* ctx, int n, const uint8_t* d_pack
                                 int16_t* d_pcm, uint8_t* d_is_comfort_noise /* may be NULL */);
 int lyra_b200_encode_dtx_device(lyra_b200_ctx* ctx, int n, const int16_t* d_pcm, int num_bits, uint8_t* d_packets,
                                 uint8_t* d_is_noise /* [n], 1 = empty packet */);
+/* The plugin surface on device memory: the twins of extract_features, quantize, dequantize, generate, logmel, noise_estimate,
+ * cng_generate and resample, for a caller that keeps features, packets, spectra or audio on the GPU between its own stages (for
+ * example its own model in place of one Lyra component).  Each takes the arguments, row sizes and return codes of its host-buffer
+ * twin, with streams 0..n-1 and every buffer a device pointer, and has the contract above: queued on the installed stream, no
+ * host wait, rows [0, n) only, LYRA_B200_EINVAL with nothing queued for a bad argument.  Role checks are the twins':
+ * extract_features_device needs the encoder role, generate_device the decoder role, the others work in any context.  Like their
+ * twins they run at 16 kHz on 320-sample rows (lyra_b200_set_sample_rate and the per-stream rate, bits and DTX words do not apply)
+ * and advance the same state: the encoder or decoder networks and hop counters, the chosen log-mel bank, the comfort-noise
+ * generators (lyra_b200_set_cng_seed and the streams' keys apply), the resampler's delay lines of that direction;
+ * generate_device follows lyra_b200_set_decoder_mode.  extract_features_device and generate_device split dense calls over many
+ * tiles into sub-batches like the codec calls (lyra_b200_set_split); results do not depend on the split.  None of them
+ * allocates or reads the context's staging buffers. */
+int lyra_b200_extract_features_device(lyra_b200_ctx* ctx, int n, const int16_t* d_pcm /* [n][320] */, float* d_features /* [n][64] */);
+int lyra_b200_quantize_device(lyra_b200_ctx* ctx, int n, const float* d_features, int num_bits, uint8_t* d_packets,
+                              int32_t* d_indices /* [n][46] or NULL */);
+int lyra_b200_dequantize_device(lyra_b200_ctx* ctx, int n, const uint8_t* d_packets, int num_bits, float* d_features);
+int lyra_b200_generate_device(lyra_b200_ctx* ctx, int n, const float* d_features /* [n][64] */, int16_t* d_pcm /* [n][320] */);
+int lyra_b200_logmel_device(lyra_b200_ctx* ctx, int bank, int n, const int16_t* d_pcm, int num_mel_bins, float* d_out);
+/* either output may be NULL, not both */
+int lyra_b200_noise_estimate_device(lyra_b200_ctx* ctx, int n, float* d_noise_estimate /* [n][160] or NULL */,
+                                    uint8_t* d_is_noise /* [n] or NULL */);
+int lyra_b200_cng_generate_device(lyra_b200_ctx* ctx, int n, const float* d_features /* [n][160] */, int16_t* d_pcm /* [n][320] */);
+/* d_in[n][in_samples] -> d_out[n][out_stride]: the first d_out_counts[k] samples of row k are written, the rest of the row is
+ * left as it is.  d_out_counts[n] (may be NULL) is written on the device; the host twin reads its counts back, which needs a
+ * synchronisation, so this twin leaves them there. */
+int lyra_b200_resample_device(lyra_b200_ctx* ctx, int to_internal, int n, int external_rate_hz, const int16_t* d_in, int in_samples,
+                              int16_t* d_out, int out_stride, int32_t* d_out_counts /* [n] or NULL */);
 /* Streams that sit out a hop: d_active is a device buffer the caller owns (NULL uninstalls it).  Like lyra_b200_set_stream this
  * is a host-side setting: every later encode_device, encode_dtx_device, decode_device, decode_track_noise_device and
  * decode_plc_device reads rows [0, n) of the buffer, in stream order on the installed stream, when its kernels run - so a server
@@ -320,7 +347,8 @@ int lyra_b200_encode_dtx_device(lyra_b200_ctx* ctx, int n, const int16_t* d_pcm,
  *   decode_track_noise_device a zero PCM row and its estimator's current is_noise, without feeding it; decode_plc_device a zero
  *   PCM row and is_comfort_noise of its unchanged state.  Any other byte runs the stream as usual.
  *   The host-buffer calls ignore the mask (their stream_ids say which streams run), as do noise_update_device (it has its own
- *   update mask) and the plugin-level calls.
+ *   update mask) and the plugin-level calls and their twins: extract_features_device, quantize_device, dequantize_device,
+ *   generate_device, logmel_device, noise_estimate_device, cng_generate_device and resample_device.
  * With no mask installed the calls launch exactly what they launch without it; with one they launch the same number of kernels,
  * and an all-ones mask gives bit-identical results.  A stream that sits out falls behind its tile neighbours' hop counters, as
  * after DTX or comfort-noise hops: lyra_b200_align_streams puts it back on a neighbour's phase.  LYRA_B200_EINVAL only for a

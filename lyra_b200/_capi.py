@@ -90,6 +90,14 @@ class CApi:
             "lyra_b200_import_streams": (ci, [vp, vp, ci, vp]),
             "lyra_b200_copy_streams": (ci, [vp, vp, vp, ci]),
             "lyra_b200_align_streams": (ci, [vp, vp, vp, ci]),
+            "lyra_b200_extract_features_device": (ci, [vp, ci, vp, vp]),
+            "lyra_b200_quantize_device": (ci, [vp, ci, vp, ci, vp, vp]),
+            "lyra_b200_dequantize_device": (ci, [vp, ci, vp, ci, vp]),
+            "lyra_b200_generate_device": (ci, [vp, ci, vp, vp]),
+            "lyra_b200_logmel_device": (ci, [vp, ci, ci, vp, ci, vp]),
+            "lyra_b200_noise_estimate_device": (ci, [vp, ci, vp, vp]),
+            "lyra_b200_cng_generate_device": (ci, [vp, ci, vp, vp]),
+            "lyra_b200_resample_device": (ci, [vp, ci, ci, ci, vp, ci, vp, ci, vp]),
         }
         for name, (res, args) in sig.items():
             fn = getattr(L, name)   # AttributeError here = the library does not export the declared ABI
@@ -109,7 +117,9 @@ class CApi:
                "lyra_b200_encode_dtx", "lyra_b200_encode_dtx_device", "lyra_b200_set_active_mask", "lyra_b200_resample", "lyra_b200_set_sample_rate",
                "lyra_b200_sample_rate", "lyra_b200_set_stream_sample_rates", "lyra_b200_stream_sample_rates", "lyra_b200_set_stream_bits",
                "lyra_b200_stream_bits", "lyra_b200_set_stream_dtx", "lyra_b200_stream_dtx", "lyra_b200_stream_state_bytes", "lyra_b200_export_streams", "lyra_b200_import_streams",
-               "lyra_b200_copy_streams", "lyra_b200_align_streams"]
+               "lyra_b200_copy_streams", "lyra_b200_align_streams", "lyra_b200_extract_features_device", "lyra_b200_quantize_device",
+               "lyra_b200_dequantize_device", "lyra_b200_generate_device", "lyra_b200_logmel_device", "lyra_b200_noise_estimate_device",
+               "lyra_b200_cng_generate_device", "lyra_b200_resample_device"]
 
 
 _product = None
@@ -463,6 +473,34 @@ class Context:
     def decode_device(self, n, d_packets, d_received, num_bits, d_pcm):
         self._check(self.api.lib.lyra_b200_decode_device(self.h, n, C.c_void_p(d_packets), C.c_void_p(d_received or 0),
                                                          num_bits, C.c_void_p(d_pcm)))
+
+    # the plugin-level calls on device buffers (streams 0..n-1, asynchronous on the installed stream; pointers as ints)
+    def extract_features_device(self, n, d_pcm, d_features):
+        self._check(self.api.lib.lyra_b200_extract_features_device(self.h, n, C.c_void_p(d_pcm), C.c_void_p(d_features)))
+
+    def quantize_device(self, n, d_features, num_bits, d_packets, d_indices=0):
+        self._check(self.api.lib.lyra_b200_quantize_device(self.h, n, C.c_void_p(d_features), num_bits, C.c_void_p(d_packets),
+                                                           C.c_void_p(d_indices or 0)))
+
+    def dequantize_device(self, n, d_packets, num_bits, d_features):
+        self._check(self.api.lib.lyra_b200_dequantize_device(self.h, n, C.c_void_p(d_packets), num_bits, C.c_void_p(d_features)))
+
+    def generate_device(self, n, d_features, d_pcm):
+        self._check(self.api.lib.lyra_b200_generate_device(self.h, n, C.c_void_p(d_features), C.c_void_p(d_pcm)))
+
+    def logmel_device(self, n, d_pcm, d_out, num_mel_bins=160, bank=0):
+        self._check(self.api.lib.lyra_b200_logmel_device(self.h, bank, n, C.c_void_p(d_pcm), num_mel_bins, C.c_void_p(d_out)))
+
+    def noise_estimate_device(self, n, d_estimate, d_is_noise):
+        self._check(self.api.lib.lyra_b200_noise_estimate_device(self.h, n, C.c_void_p(d_estimate or 0), C.c_void_p(d_is_noise or 0)))
+
+    def cng_generate_device(self, n, d_features, d_pcm):
+        self._check(self.api.lib.lyra_b200_cng_generate_device(self.h, n, C.c_void_p(d_features), C.c_void_p(d_pcm)))
+
+    def resample_device(self, n, external_rate_hz, to_internal, d_in, in_samples, d_out, out_stride, d_counts=0):
+        """Rows of in_samples -> rows of out_stride samples; the first d_counts[k] of row k are written (d_counts may be 0)."""
+        self._check(self.api.lib.lyra_b200_resample_device(self.h, 1 if to_internal else 0, n, int(external_rate_hz), C.c_void_p(d_in),
+                                                           in_samples, C.c_void_p(d_out), out_stride, C.c_void_p(d_counts or 0)))
 
     def synchronize(self):
         self._check(self.api.lib.lyra_b200_synchronize(self.h))

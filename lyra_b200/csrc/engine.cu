@@ -480,14 +480,14 @@ int ForEachPart(lyra_b200_ctx* ctx, int n, Fn body) {
   return JoinAfter(ctx, np, rc);
 }
 
-// log-mel spectra of the rows `io` into ctx->d_melout on stream `st`, advancing the extractor state `carried`
-// S: the extractor's tables by rate, used per stream at its rate (one set: Uniform; the sets share their sizes)
+// log-mel spectra of the rows `io` into `out` (by slot, num_mel floats per row) on stream `st`, advancing the extractor state
+// `carried`.  S: the extractor's tables by rate, used per stream at its rate (one set: Uniform; the sets share their sizes)
 int LaunchLogMel(lyra_b200_ctx* ctx, cudaStream_t st, const RowIo& io, const ByRate<LogMelParams>& S, const StreamWords& words,
-                 const int16_t* d_pcm, int16_t* carried, const uint8_t* d_mask) {
+                 const int16_t* d_pcm, int16_t* carried, const uint8_t* d_mask, float* out) {
   const LogMelParams& P = S.p[0];
   const size_t smem = sizeof(double) * (size_t)(2 * kLogMelFftPadded + P.fft / 2 + 1 + P.window_len + P.window_len / 8 + 1);
   return LAUNCH(6, LogMelKernel, dim3((unsigned)io.slots), dim3(kLogMelThreads), smem, st,
-                ctx->d_blob, S, words, io, d_pcm, carried, ctx->d_melout, d_mask);
+                ctx->d_blob, S, words, io, d_pcm, carried, out, d_mask);
 }
 
 // log-mel of this hop (the estimator's own extractor, bank 2) + the estimator recurrences for the rows `io` on stream `st`.
@@ -498,19 +498,20 @@ int LaunchLogMel(lyra_b200_ctx* ctx, cudaStream_t st, const RowIo& io, const ByR
 int LaunchNoiseUpdate(lyra_b200_ctx* ctx, cudaStream_t st, const RowIo& io, const StreamWords& words, bool encoder_side,
                       const int16_t* d_pcm, const uint8_t* d_mask, uint8_t* d_is_noise, float* d_estimate) {
   const int rc = LaunchLogMel(ctx, st, io, encoder_side ? ctx->enc_logmel : Uniform(ctx->spec.logmel160), words, d_pcm,
-                              encoder_side ? ctx->d_logmel_prev_enc : ctx->d_logmel_prev[2], d_mask);
+                              encoder_side ? ctx->d_logmel_prev_enc : ctx->d_logmel_prev[2], d_mask, ctx->d_melout);
   return rc ? rc : LAUNCH(7, NoiseEstimatorKernel, dim3((unsigned)io.slots), dim3(kNoiseThreads), sizeof(float) * (size_t)(2 * 160 + 2), st,
                           encoder_side ? ctx->enc_noise_params : Uniform(ctx->noise_params), words, io, ctx->d_melout, d_mask,
                           encoder_side ? ctx->d_noise_enc : ctx->d_noise, d_is_noise, d_estimate, encoder_side);
 }
 
-// comfort noise of the rows `io` into ctx->d_cng_pcm on stream `st`: from `d_features` (log-mel by slot) or, when that is
-// nullptr, from the streams' noise estimates; d_plan (by slot, nullptr: every slot) selects the slots that need it
-int LaunchComfortNoise(lyra_b200_ctx* ctx, cudaStream_t st, const RowIo& io, const float* d_features, const uint8_t* d_plan) {
+// comfort noise of the rows `io` into `out` (by slot, 320 samples per row) on stream `st`: from `d_features` (log-mel by slot)
+// or, when that is nullptr, from the streams' noise estimates; d_plan (by slot, nullptr: every slot) selects the slots that need it
+int LaunchComfortNoise(lyra_b200_ctx* ctx, cudaStream_t st, const RowIo& io, const float* d_features, const uint8_t* d_plan,
+                       int16_t* out) {
   const size_t smem = sizeof(double) * (size_t)(4 * kLogMelFftPadded + 160);
   return LAUNCH(kNoProf, ComfortNoiseKernel, dim3((unsigned)io.slots), dim3(kCngThreads), smem, st,
                 ctx->d_blob, ctx->spec.cng, io, d_features, ctx->d_noise, NoiseStateUnits(ctx->noise_params.nf),
-                d_plan, ctx->d_cng_work, ctx->d_cng_hops, ctx->cng_seed, ctx->d_cng_pcm);
+                d_plan, ctx->d_cng_work, ctx->d_cng_hops, ctx->cng_seed, out);
 }
 
 // The codec path's sample-rate converter for the rows `io` on stream `st`: dir 0 converts the external-rate rows `in`
@@ -652,7 +653,7 @@ int RunDecodePlc(lyra_b200_ctx* ctx, const CodecCall& c) {
       CU(cudaMemcpyAsync(ctx->d_packets + (size_t)p.slot0 * pb, h.packets_in + (size_t)p.slot0 * pb, pb * (size_t)p.nslots, cudaMemcpyHostToDevice, p.st));
     if ((rc = LaunchDequantize(ctx, p.st, io, c.words, d.packets_in, d.received, c.num_bits, ctx->d_features, nullptr))) return rc;
     if ((rc = LaunchDecoderNets(ctx, p, ctx->d_skip, ctx->d_features, ctx->d_model_pcm, nullptr))) return rc;
-    if ((rc = LaunchComfortNoise(ctx, p.st, planned, nullptr, ctx->d_plan))) return rc;
+    if ((rc = LaunchComfortNoise(ctx, p.st, planned, nullptr, ctx->d_plan, ctx->d_cng_pcm))) return rc;
     if ((rc = LAUNCH(kNoProf, PlcMixKernel, dim3((unsigned)p.nslots), dim3(320), (size_t)0, p.st,
                      ctx->d_blob, ctx->spec.cng, planned, ctx->d_plan, ctx->d_fade0, ctx->d_dir, ctx->d_model_pcm, ctx->d_cng_pcm, pcm16)))
       return rc;
@@ -1036,6 +1037,86 @@ int ReadStreamWords(lyra_b200_ctx* ctx, const int32_t* ids, int n, const int* wo
 int BitsRole(lyra_b200_ctx* ctx, int role) {
   if (role != LYRA_B200_ROLE_ENCODER && role != LYRA_B200_ROLE_DECODER) { ctx->err = "role must be LYRA_B200_ROLE_ENCODER or _DECODER"; return -1; }
   return RoleOk(ctx, role) ? role - 1 : -1;
+}
+
+// ---- the plugin-level calls (extract_features, quantize, dequantize, generate, logmel, noise_estimate, cng_generate, resample) ----
+// Each call is a Check*, which validates the call (role, arguments, stream ids) and queues nothing when it fails, and a Launch*,
+// which queues the call's kernels on device pointers.  A host-buffer call copies its inputs into the context's staging between the
+// two and copies its results out and synchronises after them; its *_device twin launches on the caller's buffers (rows 0..n-1)
+// and returns.  The calls run every stream at 16 kHz and read no per-stream word, nor the active mask.
+
+// the ids of a call (n in range; nullptr: streams 0..n-1) and, for a sparse host-buffer call, their device copy in *d_ids
+int StageIds(lyra_b200_ctx* ctx, const int32_t* ids, int n, const int** d_ids) {
+  const int rc = CheckIds(ctx, ids, n, false);
+  return rc ? rc : UploadIds(ctx, ids, n, d_ids);
+}
+
+// extract_features (encoder role) / generate (decoder role): the role and the call's tile map
+int CheckNets(lyra_b200_ctx* ctx, int role, const int32_t* ids, int n) {
+  ENTER(role);
+  return PrepareMap(ctx, ids, n);
+}
+
+// quantize / dequantize: any context, a bit count the codec calls accept, streams 0..n-1
+int CheckRvq(lyra_b200_ctx* ctx, int n, int num_bits) {
+  ENTER(0);
+  if (!BitsOk(ctx, num_bits)) return LYRA_B200_EINVAL;
+  return CheckIds(ctx, nullptr, n, false);
+}
+int LaunchQuantizeCall(lyra_b200_ctx* ctx, int n, const float* d_features, int num_bits, uint8_t* d_packets, int* d_indices) {
+  return LaunchQuantize(ctx, ctx->stream, Rows(WholeCall(ctx, n), nullptr, nullptr), StreamWords{}, d_features, num_bits, d_packets,
+                        d_indices, nullptr);
+}
+int LaunchDequantizeCall(lyra_b200_ctx* ctx, int n, const uint8_t* d_packets, int num_bits, float* d_features) {
+  return LaunchDequantize(ctx, ctx->stream, Rows(WholeCall(ctx, n), nullptr, nullptr), StreamWords{}, d_packets, nullptr, num_bits,
+                          d_features, nullptr);
+}
+
+// logmel: any context, bank 0 or 1, 160 or 64 bins
+int CheckLogMel(lyra_b200_ctx* ctx, int bank, const int32_t* ids, int n, int num_mel_bins, const int** d_ids) {
+  ENTER(0);
+  if (bank < 0 || bank > 1) { ctx->err = "log-mel bank must be 0 or 1"; return LYRA_B200_EINVAL; }
+  if (num_mel_bins != 160 && num_mel_bins != 64) { ctx->err = "log-mel supports 160 or 64 mel bins"; return LYRA_B200_EINVAL; }
+  return StageIds(ctx, ids, n, d_ids);
+}
+int LaunchLogMelCall(lyra_b200_ctx* ctx, int bank, const int* d_ids, int n, const int16_t* d_pcm, int num_mel_bins, float* d_out) {
+  const LogMelParams& P = num_mel_bins == 160 ? ctx->spec.logmel160 : ctx->spec.logmel64;
+  return LaunchLogMel(ctx, ctx->stream, Rows(WholeCall(ctx, n), d_ids, nullptr), Uniform(P), kWords16k, d_pcm, ctx->d_logmel_prev[bank],
+                      nullptr, d_out);
+}
+
+// noise_estimate / cng_generate: any context
+int CheckRows(lyra_b200_ctx* ctx, const int32_t* ids, int n, const int** d_ids) {
+  ENTER(0);
+  return StageIds(ctx, ids, n, d_ids);
+}
+int LaunchNoiseRead(lyra_b200_ctx* ctx, const int* d_ids, int n, float* d_estimate, uint8_t* d_is_noise) {
+  return LAUNCH(kNoProf, NoiseReadKernel, dim3((unsigned)n), dim3(192), (size_t)0, ctx->stream,
+                Rows(WholeCall(ctx, n), d_ids, nullptr), ctx->d_noise, ctx->noise_params.nf, d_estimate, d_is_noise);
+}
+
+// resample: any context, a supported rate, at most 960 samples in and out per row and room for all outputs; *pr = the filter pair
+int CheckResample(lyra_b200_ctx* ctx, int to_internal, const int32_t* ids, int n, int external_rate_hz, int in_samples, int out_stride,
+                  int* pr, const int** d_ids) {
+  ENTER(0);
+  const int pair = RatePair(external_rate_hz);
+  if (pair < 0) { ctx->err = "the resampler converts between 16 kHz and 8 / 32 / 48 kHz"; return LYRA_B200_EINVAL; }
+  *pr = to_internal ? pair : pair + 3;
+  const int num = ctx->spec.resampler.num[*pr], den = ctx->spec.resampler.den[*pr];
+  const int max_out = (in_samples * den + num - 1) / num;
+  if (in_samples <= 0 || in_samples > 960 || max_out > 960 || out_stride < max_out || out_stride > 968) {
+    ctx->err = "resample: at most 960 input and 960 output samples per stream and call, and room for ceil(n * out / in) outputs";
+    return LYRA_B200_EINVAL;
+  }
+  return StageIds(ctx, ids, n, d_ids);
+}
+// rows of in_samples inputs -> rows of out_stride outputs, of which the first counts[slot] (counts may be nullptr) are written
+int LaunchResampleCall(lyra_b200_ctx* ctx, int pr, int to_internal, int external_rate_hz, const int* d_ids, int n, const int16_t* d_in,
+                       int in_samples, int16_t* d_out, int out_stride, int* d_counts) {
+  const int dir = to_internal ? 0 : 1;
+  return LAUNCH(kNoProf, ResampleKernel, dim3((unsigned)n), dim3(128), sizeof(float) * (size_t)(kResamplerTaps - 1 + in_samples),
+                ctx->stream, ctx->d_blob, ctx->spec.resampler, pr, external_rate_hz, Rows(WholeCall(ctx, n), d_ids, nullptr),
+                StreamWords{}, d_in, in_samples, in_samples, d_out, out_stride, d_counts, ctx->d_rs_delay[dir], ctx->d_rs_pos[dir]);
 }
 
 }  // namespace
@@ -1484,8 +1565,7 @@ int lyra_b200_decode(lyra_b200_ctx* ctx, const int32_t* ids, int n, const uint8_
 
 int lyra_b200_extract_features(lyra_b200_ctx* ctx, const int32_t* ids, int n, const int16_t* pcm, float* features) {
   if (!ctx || !pcm || !features) return LYRA_B200_EINVAL;
-  ENTER(LYRA_B200_ROLE_ENCODER);
-  int rc = PrepareMap(ctx, ids, n);
+  int rc = CheckNets(ctx, LYRA_B200_ROLE_ENCODER, ids, n);
   if (rc) return rc;
   CU(cudaMemcpyAsync(ctx->d_pcm, pcm, sizeof(int16_t) * 320 * (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
   if ((rc = LaunchEncoderNets(ctx, WholeCall(ctx, n), nullptr, ctx->d_pcm, ctx->d_features, nullptr))) return rc;
@@ -1494,41 +1574,50 @@ int lyra_b200_extract_features(lyra_b200_ctx* ctx, const int32_t* ids, int n, co
   return LYRA_B200_OK;
 }
 
+int lyra_b200_extract_features_device(lyra_b200_ctx* ctx, int n, const int16_t* d_pcm, float* d_features) {
+  if (!ctx || !d_pcm || !d_features) return LYRA_B200_EINVAL;
+  const int rc = CheckNets(ctx, LYRA_B200_ROLE_ENCODER, nullptr, n);
+  return rc ? rc : ForEachPart(ctx, n, [&](const Part& p) { return LaunchEncoderNets(ctx, p, nullptr, d_pcm, d_features, nullptr); });
+}
+
 int lyra_b200_quantize(lyra_b200_ctx* ctx, int n, const float* features, int num_bits, uint8_t* packets, int32_t* indices) {
   if (!ctx || !features || !packets) return LYRA_B200_EINVAL;
-  ENTER(0);
-  if (!BitsOk(ctx, num_bits)) return LYRA_B200_EINVAL;
-  int rc = CheckIds(ctx, nullptr, n, false);
+  int rc = CheckRvq(ctx, n, num_bits);
   if (rc) return rc;
   CU(cudaMemcpyAsync(ctx->d_features, features, sizeof(float) * 64 * (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
-  rc = LaunchQuantize(ctx, ctx->stream, Rows(WholeCall(ctx, n), nullptr, nullptr), StreamWords{}, ctx->d_features, num_bits, ctx->d_packets,
-                      indices ? ctx->d_indices : nullptr, nullptr);
-  if (rc) return rc;
+  if ((rc = LaunchQuantizeCall(ctx, n, ctx->d_features, num_bits, ctx->d_packets, indices ? ctx->d_indices : nullptr))) return rc;
   CU(cudaMemcpyAsync(packets, ctx->d_packets, (size_t)PacketBytes(num_bits) * (size_t)n, cudaMemcpyDeviceToHost, ctx->stream));
   if (indices) CU(cudaMemcpyAsync(indices, ctx->d_indices, sizeof(int) * 46 * (size_t)n, cudaMemcpyDeviceToHost, ctx->stream));
   CU(SyncStream(ctx));
   return LYRA_B200_OK;
 }
 
+int lyra_b200_quantize_device(lyra_b200_ctx* ctx, int n, const float* d_features, int num_bits, uint8_t* d_packets, int32_t* d_indices) {
+  if (!ctx || !d_features || !d_packets) return LYRA_B200_EINVAL;
+  const int rc = CheckRvq(ctx, n, num_bits);
+  return rc ? rc : LaunchQuantizeCall(ctx, n, d_features, num_bits, d_packets, d_indices);
+}
+
 int lyra_b200_dequantize(lyra_b200_ctx* ctx, int n, const uint8_t* packets, int num_bits, float* features) {
   if (!ctx || !features || !packets) return LYRA_B200_EINVAL;
-  ENTER(0);
-  if (!BitsOk(ctx, num_bits)) return LYRA_B200_EINVAL;
-  int rc = CheckIds(ctx, nullptr, n, false);
+  int rc = CheckRvq(ctx, n, num_bits);
   if (rc) return rc;
   CU(cudaMemcpyAsync(ctx->d_packets, packets, (size_t)PacketBytes(num_bits) * (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
-  rc = LaunchDequantize(ctx, ctx->stream, Rows(WholeCall(ctx, n), nullptr, nullptr), StreamWords{}, ctx->d_packets, nullptr, num_bits,
-                        ctx->d_features, nullptr);
-  if (rc) return rc;
+  if ((rc = LaunchDequantizeCall(ctx, n, ctx->d_packets, num_bits, ctx->d_features))) return rc;
   CU(cudaMemcpyAsync(features, ctx->d_features, sizeof(float) * 64 * (size_t)n, cudaMemcpyDeviceToHost, ctx->stream));
   CU(SyncStream(ctx));
   return LYRA_B200_OK;
 }
 
+int lyra_b200_dequantize_device(lyra_b200_ctx* ctx, int n, const uint8_t* d_packets, int num_bits, float* d_features) {
+  if (!ctx || !d_packets || !d_features) return LYRA_B200_EINVAL;
+  const int rc = CheckRvq(ctx, n, num_bits);
+  return rc ? rc : LaunchDequantizeCall(ctx, n, d_packets, num_bits, d_features);
+}
+
 int lyra_b200_generate(lyra_b200_ctx* ctx, const int32_t* ids, int n, const float* features, int16_t* pcm) {
   if (!ctx || !features || !pcm) return LYRA_B200_EINVAL;
-  ENTER(LYRA_B200_ROLE_DECODER);
-  int rc = PrepareMap(ctx, ids, n);
+  int rc = CheckNets(ctx, LYRA_B200_ROLE_DECODER, ids, n);
   if (rc) return rc;
   CU(cudaMemcpyAsync(ctx->d_features, features, sizeof(float) * 64 * (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
   if ((rc = LaunchDecoderNets(ctx, WholeCall(ctx, n), nullptr, ctx->d_features, ctx->d_pcm, nullptr))) return rc;
@@ -1537,22 +1626,29 @@ int lyra_b200_generate(lyra_b200_ctx* ctx, const int32_t* ids, int n, const floa
   return LYRA_B200_OK;
 }
 
+int lyra_b200_generate_device(lyra_b200_ctx* ctx, int n, const float* d_features, int16_t* d_pcm) {
+  if (!ctx || !d_features || !d_pcm) return LYRA_B200_EINVAL;
+  const int rc = CheckNets(ctx, LYRA_B200_ROLE_DECODER, nullptr, n);
+  return rc ? rc : ForEachPart(ctx, n, [&](const Part& p) { return LaunchDecoderNets(ctx, p, nullptr, d_features, d_pcm, nullptr); });
+}
+
 int lyra_b200_logmel(lyra_b200_ctx* ctx, int bank, const int32_t* ids, int n, const int16_t* pcm, int num_mel_bins, float* out) {
   if (!ctx || !pcm || !out) return LYRA_B200_EINVAL;
-  ENTER(0);
-  if (bank < 0 || bank > 1) { ctx->err = "log-mel bank must be 0 or 1"; return LYRA_B200_EINVAL; }
-  if (num_mel_bins != 160 && num_mel_bins != 64) { ctx->err = "log-mel supports 160 or 64 mel bins"; return LYRA_B200_EINVAL; }
   const int* d_ids = nullptr;
-  int rc = CheckIds(ctx, ids, n, false);
-  if (rc || (rc = UploadIds(ctx, ids, n, &d_ids))) return rc;
-  const LogMelParams& P = num_mel_bins == 160 ? ctx->spec.logmel160 : ctx->spec.logmel64;
+  int rc = CheckLogMel(ctx, bank, ids, n, num_mel_bins, &d_ids);
+  if (rc) return rc;
   CU(cudaMemcpyAsync(ctx->d_pcm, pcm, sizeof(int16_t) * 320 * (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
-  if ((rc = LaunchLogMel(ctx, ctx->stream, Rows(WholeCall(ctx, n), d_ids, nullptr), Uniform(P), kWords16k, ctx->d_pcm,
-                         ctx->d_logmel_prev[bank], nullptr)))
-    return rc;
+  if ((rc = LaunchLogMelCall(ctx, bank, d_ids, n, ctx->d_pcm, num_mel_bins, ctx->d_melout))) return rc;
   CU(cudaMemcpyAsync(out, ctx->d_melout, sizeof(float) * (size_t)num_mel_bins * (size_t)n, cudaMemcpyDeviceToHost, ctx->stream));
   CU(SyncStream(ctx));
   return LYRA_B200_OK;
+}
+
+int lyra_b200_logmel_device(lyra_b200_ctx* ctx, int bank, int n, const int16_t* d_pcm, int num_mel_bins, float* d_out) {
+  if (!ctx || !d_pcm || !d_out) return LYRA_B200_EINVAL;
+  const int* d_ids = nullptr;
+  const int rc = CheckLogMel(ctx, bank, nullptr, n, num_mel_bins, &d_ids);
+  return rc ? rc : LaunchLogMelCall(ctx, bank, nullptr, n, d_pcm, num_mel_bins, d_out);
 }
 
 int lyra_b200_noise_update(lyra_b200_ctx* ctx, const int32_t* ids, int n, const int16_t* pcm, const uint8_t* update_mask,
@@ -1687,39 +1783,34 @@ int lyra_b200_set_cng_seed(lyra_b200_ctx* ctx, uint64_t seed) {
 
 int lyra_b200_cng_generate(lyra_b200_ctx* ctx, const int32_t* ids, int n, const float* features, int16_t* pcm) {
   if (!ctx || !features || !pcm) return LYRA_B200_EINVAL;
-  ENTER(0);
   const int* d_ids = nullptr;
-  int rc = CheckIds(ctx, ids, n, false);
-  if (rc || (rc = UploadIds(ctx, ids, n, &d_ids))) return rc;
+  int rc = CheckRows(ctx, ids, n, &d_ids);
+  if (rc) return rc;
   CU(cudaMemcpyAsync(ctx->d_cng_feat, features, sizeof(float) * 160 * (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
-  if ((rc = LaunchComfortNoise(ctx, ctx->stream, Rows(WholeCall(ctx, n), d_ids, nullptr), ctx->d_cng_feat, nullptr))) return rc;
+  if ((rc = LaunchComfortNoise(ctx, ctx->stream, Rows(WholeCall(ctx, n), d_ids, nullptr), ctx->d_cng_feat, nullptr, ctx->d_cng_pcm)))
+    return rc;
   CU(cudaMemcpyAsync(pcm, ctx->d_cng_pcm, sizeof(int16_t) * 320 * (size_t)n, cudaMemcpyDeviceToHost, ctx->stream));
   CU(SyncStream(ctx));
   return LYRA_B200_OK;
 }
 
+int lyra_b200_cng_generate_device(lyra_b200_ctx* ctx, int n, const float* d_features, int16_t* d_pcm) {
+  if (!ctx || !d_features || !d_pcm) return LYRA_B200_EINVAL;
+  const int* d_ids = nullptr;
+  const int rc = CheckRows(ctx, nullptr, n, &d_ids);
+  return rc ? rc : LaunchComfortNoise(ctx, ctx->stream, Rows(WholeCall(ctx, n), nullptr, nullptr), d_features, nullptr, d_pcm);
+}
+
 int lyra_b200_resample(lyra_b200_ctx* ctx, int to_internal, const int32_t* ids, int n, int external_rate_hz, const int16_t* in,
                        int in_samples, int16_t* out, int out_stride, int32_t* out_counts) {
   if (!ctx || !in || !out) return LYRA_B200_EINVAL;
-  ENTER(0);
-  const int pair = RatePair(external_rate_hz);
-  if (pair < 0) { ctx->err = "the resampler converts between 16 kHz and 8 / 32 / 48 kHz"; return LYRA_B200_EINVAL; }
-  const int pr = to_internal ? pair : pair + 3;
-  const int num = ctx->spec.resampler.num[pr], den = ctx->spec.resampler.den[pr];
-  const int max_out = (in_samples * den + num - 1) / num;
-  if (in_samples <= 0 || in_samples > 960 || max_out > 960 || out_stride < max_out || out_stride > 968) {
-    ctx->err = "resample: at most 960 input and 960 output samples per stream and call, and room for ceil(n * out / in) outputs";
-    return LYRA_B200_EINVAL;
-  }
   const int* d_ids = nullptr;
-  int rc = CheckIds(ctx, ids, n, false);
-  if (rc || (rc = UploadIds(ctx, ids, n, &d_ids))) return rc;
+  int pr = 0;
+  int rc = CheckResample(ctx, to_internal, ids, n, external_rate_hz, in_samples, out_stride, &pr, &d_ids);
+  if (rc) return rc;
   CU(cudaMemcpyAsync(ctx->d_rs_in, in, sizeof(int16_t) * (size_t)in_samples * (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
-  const int dir = to_internal ? 0 : 1;
-  if ((rc = LAUNCH(kNoProf, ResampleKernel, dim3((unsigned)n), dim3(128), sizeof(float) * (size_t)(kResamplerTaps - 1 + in_samples),
-                   ctx->stream, ctx->d_blob, ctx->spec.resampler, pr, external_rate_hz, Rows(WholeCall(ctx, n), d_ids, nullptr),
-                   StreamWords{}, ctx->d_rs_in, in_samples, in_samples, ctx->d_rs_out, out_stride, ctx->d_rs_counts, ctx->d_rs_delay[dir],
-                   ctx->d_rs_pos[dir])))
+  if ((rc = LaunchResampleCall(ctx, pr, to_internal, external_rate_hz, d_ids, n, ctx->d_rs_in, in_samples, ctx->d_rs_out, out_stride,
+                               ctx->d_rs_counts)))
     return rc;
   CU(cudaMemcpyAsync(out, ctx->d_rs_out, sizeof(int16_t) * (size_t)out_stride * (size_t)n, cudaMemcpyDeviceToHost, ctx->stream));
   std::vector<int> counts((size_t)n);
@@ -1727,6 +1818,15 @@ int lyra_b200_resample(lyra_b200_ctx* ctx, int to_internal, const int32_t* ids, 
   CU(SyncStream(ctx));
   if (out_counts) for (int k = 0; k < n; ++k) out_counts[k] = counts[(size_t)k];
   return LYRA_B200_OK;
+}
+
+int lyra_b200_resample_device(lyra_b200_ctx* ctx, int to_internal, int n, int external_rate_hz, const int16_t* d_in, int in_samples,
+                              int16_t* d_out, int out_stride, int32_t* d_out_counts) {
+  if (!ctx || !d_in || !d_out) return LYRA_B200_EINVAL;
+  const int* d_ids = nullptr;
+  int pr = 0;
+  const int rc = CheckResample(ctx, to_internal, nullptr, n, external_rate_hz, in_samples, out_stride, &pr, &d_ids);
+  return rc ? rc : LaunchResampleCall(ctx, pr, to_internal, external_rate_hz, nullptr, n, d_in, in_samples, d_out, out_stride, d_out_counts);
 }
 
 int lyra_b200_stream_state_bytes(const lyra_b200_ctx* ctx) { return ctx ? (int)RecordBytes(ctx) : 0; }
@@ -1825,18 +1925,21 @@ int lyra_b200_align_streams(lyra_b200_ctx* ctx, const int32_t* stream_ids, const
 
 int lyra_b200_noise_estimate(lyra_b200_ctx* ctx, const int32_t* ids, int n, float* noise_estimate, uint8_t* is_noise) {
   if (!ctx || (!noise_estimate && !is_noise)) return LYRA_B200_EINVAL;
-  ENTER(0);
   const int* d_ids = nullptr;
-  int rc = CheckIds(ctx, ids, n, false);
-  if (rc || (rc = UploadIds(ctx, ids, n, &d_ids))) return rc;
-  if ((rc = LAUNCH(kNoProf, NoiseReadKernel, dim3((unsigned)n), dim3(192), (size_t)0, ctx->stream,
-                   Rows(WholeCall(ctx, n), d_ids, nullptr), ctx->d_noise, ctx->noise_params.nf, noise_estimate ? ctx->d_noise_est : nullptr,
-                   is_noise ? ctx->d_is_noise : nullptr)))
+  int rc = CheckRows(ctx, ids, n, &d_ids);
+  if (rc || (rc = LaunchNoiseRead(ctx, d_ids, n, noise_estimate ? ctx->d_noise_est : nullptr, is_noise ? ctx->d_is_noise : nullptr)))
     return rc;
   if (noise_estimate) CU(cudaMemcpyAsync(noise_estimate, ctx->d_noise_est, sizeof(float) * 160 * (size_t)n, cudaMemcpyDeviceToHost, ctx->stream));
   if (is_noise) CU(cudaMemcpyAsync(is_noise, ctx->d_is_noise, (size_t)n, cudaMemcpyDeviceToHost, ctx->stream));
   CU(SyncStream(ctx));
   return LYRA_B200_OK;
+}
+
+int lyra_b200_noise_estimate_device(lyra_b200_ctx* ctx, int n, float* d_noise_estimate, uint8_t* d_is_noise) {
+  if (!ctx || (!d_noise_estimate && !d_is_noise)) return LYRA_B200_EINVAL;
+  const int* d_ids = nullptr;
+  const int rc = CheckRows(ctx, nullptr, n, &d_ids);
+  return rc ? rc : LaunchNoiseRead(ctx, nullptr, n, d_noise_estimate, d_is_noise);
 }
 
 }  // extern "C"
