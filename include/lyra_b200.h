@@ -354,6 +354,53 @@ int lyra_b200_resample_device(lyra_b200_ctx* ctx, int to_internal, int n, int ex
  * after DTX or comfort-noise hops: lyra_b200_align_streams puts it back on a neighbour's phase.  LYRA_B200_EINVAL only for a
  * NULL context; works in any context. */
 int lyra_b200_set_active_mask(lyra_b200_ctx* ctx, const uint8_t* d_active);
+/* Per-stream call statistics on the device: audio level (RFC 6464 / RFC 6465), energy, DTX and concealment counters, per role.
+ * A stream's statistics in one role are LYRA_B200_STATS_WORDS uint64 words; indices 4-6 mean different things per role:
+ *   HOPS      calls in which the stream ran (the fused codec calls of the role; hops it sat out are not counted)
+ *   SAT_OUT   *_device calls in which the active mask (lyra_b200_set_active_mask) sat it out
+ *   ENERGY    sum over its run hops of floor(sum of squares / hop samples), in int16^2 units (WebRTC totalAudioEnergy =
+ *             ENERGY * 0.02 / 2^30)
+ *   LEVEL     RFC 6464 level of its last run hop, 0..127 (-dBov); 127 before any hop
+ *   encoder:  EMPTY    run hops that produced an empty DTX packet (encode_dtx)
+ *             BITS     sum of the bit counts of its non-empty packets (its own bits word, lyra_b200_set_stream_bits, or the
+ *                      call's num_bits)
+ *   decoder:  RECEIVED run hops decoded from a received packet
+ *             CN_HOPS  run hops whose output contains comfort noise, fades included (decode_plc only)
+ *             EVENTS   concealment events: a run hop that is not received and follows a received run hop, or is the stream's
+ *                      first run hop
+ * Unused words read 0.  The level and energy are taken over the stream's own hop at the external rate: the first rate / 50
+ * samples of its row, the encoder's input row or the decoder's output row; DTX-empty hops are run hops.  LEVEL is the number of
+ * thresholds t_k = 2^30 * 10^(-(k + 0.5) / 10), k = 0..126, computed on the host, that exceed (double)sum_of_squares / samples:
+ * digital silence gives 127 and a full-scale square wave 0.
+ *   lyra_b200_set_stats is a host-side setting like the active mask (no queue drain; 0 by default).  While it is 0 every call
+ *   launches exactly what it launches without it and no statistic moves.  While it is 1 each of encode, encode_dtx, decode,
+ *   decode_track_noise and decode_plc, host-buffer (stream_ids too) or *_device twin, launches one more kernel per sub-batch and
+ *   updates the statistics of the call's role by stream id; a stream that sits out only counts SAT_OUT and its row is not read.
+ *   The plugin-level calls and their twins, noise_update(_device) and resample(_device) do not count.  Captured graphs
+ *   (lyra_b200_set_graphs) are kept per setting.
+ *   The statistics are per-stream state: lyra_b200_reset and copy_streams from -1 restore the initial image, copy_streams,
+ *   export_streams and import_streams carry them (import refuses a LEVEL above 127).
+ *   lyra_b200_read_stats: stats[k][0..7] = the statistics of stream stream_ids[k] (NULL: k; an id may be listed more than once)
+ *   in `role`.  Ordered on the installed stream behind the work queued there; returns when the values are in the caller's
+ *   buffer.  lyra_b200_read_stats_device: the same for streams 0..n-1 into the device buffer d_stats, rows [0, n) only,
+ *   asynchronous on the installed stream like the *_device calls.  clear = 1 then zeroes the counters and the energy of the
+ *   listed streams, in stream order after reading; LEVEL and the event state stay, so a server can poll every hop or every
+ *   second without losing a hop.
+ * role is LYRA_B200_ROLE_ENCODER or LYRA_B200_ROLE_DECODER and must be a role of the context.  A bad role, n or id, or a NULL
+ * buffer returns LYRA_B200_EINVAL and queues nothing. */
+#define LYRA_B200_STATS_WORDS 8
+#define LYRA_B200_STAT_HOPS 0
+#define LYRA_B200_STAT_SAT_OUT 1
+#define LYRA_B200_STAT_ENERGY 2
+#define LYRA_B200_STAT_LEVEL 3
+#define LYRA_B200_STAT_EMPTY 4      /* encoder */
+#define LYRA_B200_STAT_BITS 5       /* encoder */
+#define LYRA_B200_STAT_RECEIVED 4   /* decoder */
+#define LYRA_B200_STAT_CN_HOPS 5    /* decoder */
+#define LYRA_B200_STAT_EVENTS 6     /* decoder */
+int lyra_b200_set_stats(lyra_b200_ctx* ctx, int enable);
+int lyra_b200_read_stats(lyra_b200_ctx* ctx, int role, const int32_t* stream_ids, int n, uint64_t* stats /* [n][8] */, int clear);
+int lyra_b200_read_stats_device(lyra_b200_ctx* ctx, int role, int n, uint64_t* d_stats /* [n][8] */, int clear);
 int lyra_b200_synchronize(lyra_b200_ctx* ctx);
 /* Dense calls (stream_ids == NULL / *_device) over many tiles are cut into `parts` (1..4, default 3) sub-batches that
  * run concurrently on internal CUDA streams so partial waves of one kernel are filled by another's blocks.

@@ -16,6 +16,11 @@ MODEL_DIR = os.path.join(_HERE, "model_coeffs")
 
 OK, EINVAL, ENODEV, EMODEL = 0, -1, -2, -3
 HOP = 320
+STATS_WORDS = 8
+# word indices of one stream's call statistics (lyra_b200_read_stats); 4-6 differ per role
+STAT_HOPS, STAT_SAT_OUT, STAT_ENERGY, STAT_LEVEL = 0, 1, 2, 3
+STAT_EMPTY, STAT_BITS = 4, 5                       # encoder
+STAT_RECEIVED, STAT_CN_HOPS, STAT_EVENTS = 4, 5, 6  # decoder
 NUM_FEATURES = 64
 MAX_STAGES = 46
 
@@ -76,6 +81,9 @@ class CApi:
             "lyra_b200_encode_dtx": (ci, [vp, vp, ci, vp, ci, vp, vp]),
             "lyra_b200_encode_dtx_device": (ci, [vp, ci, vp, ci, vp, vp]),
             "lyra_b200_set_active_mask": (ci, [vp, vp]),
+            "lyra_b200_set_stats": (ci, [vp, ci]),
+            "lyra_b200_read_stats": (ci, [vp, ci, vp, ci, vp, ci]),
+            "lyra_b200_read_stats_device": (ci, [vp, ci, ci, vp, ci]),
             "lyra_b200_resample": (ci, [vp, ci, vp, ci, ci, vp, ci, vp, ci, vp]),
             "lyra_b200_set_sample_rate": (ci, [vp, ci]),
             "lyra_b200_sample_rate": (ci, [vp]),
@@ -114,7 +122,8 @@ class CApi:
                "lyra_b200_decode_track_noise_device", "lyra_b200_set_split", "lyra_b200_set_blocking_sync", "lyra_b200_set_graphs", "lyra_b200_set_priority", "lyra_b200_graph_replays", "lyra_b200_set_decoder_mode", "lyra_b200_decoder_mode", "lyra_b200_launch_count", "lyra_b200_profile_enable",
                "lyra_b200_profile_read", "lyra_b200_noise_estimate", "lyra_b200_decode_plc", "lyra_b200_decode_plc_device",
                "lyra_b200_plc_get_state", "lyra_b200_plc_set_state", "lyra_b200_cng_generate", "lyra_b200_set_cng_seed",
-               "lyra_b200_encode_dtx", "lyra_b200_encode_dtx_device", "lyra_b200_set_active_mask", "lyra_b200_resample", "lyra_b200_set_sample_rate",
+               "lyra_b200_encode_dtx", "lyra_b200_encode_dtx_device", "lyra_b200_set_active_mask", "lyra_b200_set_stats",
+               "lyra_b200_read_stats", "lyra_b200_read_stats_device", "lyra_b200_resample", "lyra_b200_set_sample_rate",
                "lyra_b200_sample_rate", "lyra_b200_set_stream_sample_rates", "lyra_b200_stream_sample_rates", "lyra_b200_set_stream_bits",
                "lyra_b200_stream_bits", "lyra_b200_set_stream_dtx", "lyra_b200_stream_dtx", "lyra_b200_stream_state_bytes", "lyra_b200_export_streams", "lyra_b200_import_streams",
                "lyra_b200_copy_streams", "lyra_b200_align_streams", "lyra_b200_extract_features_device", "lyra_b200_quantize_device",
@@ -361,6 +370,25 @@ class Context:
         caller keeps it alive while calls that read it are queued) or None to uninstall.  Row k = 0: stream k sits the call out."""
         ptr = mask.data_ptr() if hasattr(mask, "data_ptr") else mask
         self._check(self.api.lib.lyra_b200_set_active_mask(self.h, C.c_void_p(ptr or 0)))
+
+    def set_stats(self, enable):
+        """Per-stream call statistics of the fused codec calls on (1) or off (0, the default); a host-side setting."""
+        self._check(self.api.lib.lyra_b200_set_stats(self.h, 1 if enable else 0))
+
+    def stats(self, role, stream_ids=None, n=None, clear=False):
+        """The call statistics of each listed stream in role "encoder" or "decoder" (default: streams 0..n-1, n = max_streams)
+        -> uint64[n][STATS_WORDS]; clear zeroes the counters and the energy after reading (the level and event state stay)."""
+        ids = None if stream_ids is None else np.ascontiguousarray(stream_ids, dtype=np.int32).reshape(-1)
+        n = ids.size if ids is not None else (self.max_streams if n is None else n)
+        out = np.empty((n, STATS_WORDS), dtype=np.uint64)
+        self._check(self.api.lib.lyra_b200_read_stats(self.h, self.ROLES.get(role, role), _ptr(ids), n, _ptr(out), 1 if clear else 0))
+        return out
+
+    def stats_device(self, role, n, d_out, clear=False):
+        """The call statistics of streams 0..n-1 into the device buffer d_out (uint64[n][STATS_WORDS], pointer as int);
+        asynchronous on the installed stream."""
+        self._check(self.api.lib.lyra_b200_read_stats_device(self.h, self.ROLES.get(role, role), int(n), C.c_void_p(d_out),
+                                                             1 if clear else 0))
 
     def decode_track_noise(self, packets, num_bits, stream_ids=None, received=None):
         """decode() + noise-estimator update of the received streams on the device -> (pcm[n][320], is_noise[n])."""

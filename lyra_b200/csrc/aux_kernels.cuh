@@ -199,14 +199,14 @@ enum StreamStateKind { kStatePlain = 0, kStateCodecRs0 = 1, kStateCodecRs1 = 2, 
 constexpr uint32_t kStateMagic = 0x5453594Cu;        // "LYST"
 // 2: the per-stream sample rate joined the payload; 3: the per-stream bit counts.  The per-stream DTX word kept 3: it adds a word
 // to encoder-role records only, whose size word (kHdrBytes) already refuses the shorter records, and decoder-only records did
-// not change.
+// not change.  The call statistics (one entry per role) kept 3 for the same reason: every record grew, so its size word differs.
 constexpr uint32_t kStateVersion = 3;
 constexpr int kStateHeaderWords = 16;
 // header words: magic, version, record bytes, roles, sample rate, 0, model fingerprint (lo, hi), codec converter 0 / 1 live,
 // comfort-noise key (lo, hi), 0 x 4
 enum { kHdrMagic = 0, kHdrVersion, kHdrBytes, kHdrRoles, kHdrRate, kHdrZero5, kHdrModelLo, kHdrModelHi, kHdrLive0, kHdrLive1,
        kHdrKeyLo, kHdrKeyHi };
-constexpr int kStateMaxEntries = 25;                 // a context with both roles registers exactly 25: a new per-stream entry raises it
+constexpr int kStateMaxEntries = 27;                 // a context with both roles registers exactly 27: a new per-stream entry raises it
 constexpr int kStateRows = 8;                        // rows of a call per block
 constexpr int kStateChunk = 1024;                    // rows per launch (the ids travel as kernel parameters)
 constexpr int kStateThreads = 256;

@@ -50,7 +50,7 @@ struct lyra_b200_ctx {
   // (nullptr: zero), hop counter `n18` (nullptr: none; initially 0).  `reset` = false: lyra_b200_reset leaves the entry alone
   // (lyra_b200_resample's delay lines).  `kind` (StreamStateKind) marks the words a record does not carry verbatim; `check`
   // is what import validates in a record's payload besides the hop counter.
-  enum Check { kCheckNone, kCheckPlc, kCheckResamplerPos, kCheckStreamRate, kCheckStreamBits, kCheckStreamDtx };
+  enum Check { kCheckNone, kCheckPlc, kCheckResamplerPos, kCheckStreamRate, kCheckStreamBits, kCheckStreamDtx, kCheckStats };
   struct StateEntry {
     StreamStateEntry e;              // e.offset is set by BuildStateTable
     bool reset;
@@ -130,6 +130,13 @@ struct lyra_b200_ctx {
   // lyra_b200_set_active_mask: the caller's buffer, by row of the *_device codec calls (0 = the stream sits the call out); nullptr:
   // every stream runs and the kernels get no pointer
   const uint8_t* d_active = nullptr;
+  // lyra_b200_set_stats: the fused codec calls launch CallStatsKernel once per part into d_stats[role index] (per-stream state,
+  // kStatsWords u64 per stream; nullptr when the context lacks the role).  d_stats_levels: the 128 level thresholds;
+  // d_stats_out: lyra_b200_read_stats's staging [max_streams][kStatsWords]
+  bool stats_on = false;
+  unsigned long long* d_stats[2] = {nullptr, nullptr};
+  double* d_stats_levels = nullptr;
+  unsigned long long* d_stats_out = nullptr;
   // tile map
   int* d_tile_list = nullptr;
   int* d_slot_of = nullptr;
@@ -160,14 +167,14 @@ struct lyra_b200_ctx {
   // lyra_b200_set_graphs: the dense host-buffer encode / decode calls replay a captured CUDA graph (copies in, kernels of every
   // sub-batch, copies out) instead of re-issuing ~20 stream operations per call; one graph per (call shape, host buffers)
   // (rates: rate_override, which adds the converters' launches at 16 kHz; bits: own_words of the call's role's bits word, which
-  // hands the RVQ kernels the bits words)
+  // hands the RVQ kernels the bits words; stats: stats_on, which adds CallStatsKernel's launches)
   struct GraphKey {
     int kind, n, num_bits, mode, nsplit;
     const void *a, *b, *c;
-    bool rates, bits;
+    bool rates, bits, stats;
     bool operator==(const GraphKey& o) const {
       return kind == o.kind && n == o.n && num_bits == o.num_bits && mode == o.mode && nsplit == o.nsplit && a == o.a && b == o.b && c == o.c &&
-             rates == o.rates && bits == o.bits;
+             rates == o.rates && bits == o.bits && stats == o.stats;
     }
   };
   struct GraphEntry { GraphKey key; void* exec; uint64_t launches; };
@@ -553,6 +560,17 @@ struct CodecCall {
   StreamWords words{};                     // the per-stream words of the call's role
 };
 
+// lyra_b200_set_stats: CallStatsKernel over part p's rows of `pcm` (the encoders' input rows, the decoders' output rows, at the
+// external rate) with the call's event source (StatsSource); nothing while statistics are off
+int LaunchCallStats(lyra_b200_ctx* ctx, const Part& p, const CodecCall& c, const int16_t* pcm, const uint8_t* events) {
+  if (!ctx->stats_on) return LYRA_B200_OK;
+  const bool encoder = c.kind == kEncode || c.kind == kEncodeDtx;
+  const int source = c.kind == kEncode ? kStatsEncode : c.kind == kEncodeDtx ? kStatsEncodeDtx : c.kind == kDecodePlc ? kStatsDecodePlc : kStatsDecode;
+  return LAUNCH(kNoProf, CallStatsKernel, dim3((unsigned)((p.nslots + kStatsRowsPerBlock - 1) / kStatsRowsPerBlock)), dim3(kStatsThreads),
+                (size_t)0, p.st, Rows(p, c.d_ids, c.active), c.words, pcm, ctx->sample_rate / 50, source, events, c.num_bits,
+                ctx->d_stats_levels, ctx->d_stats[encoder ? 0 : 1]);
+}
+
 // encode / encode_dtx.  PCM rows hold ctx->sample_rate / 50 samples (the external rate).  At 16 kHz the encoder reads the rows
 // (a host-buffer call's are copied to ctx->d_pcm first); at another rate every sub-batch first converts them into the 16 kHz scratch
 // ctx->d_pcm (a host-buffer call stages its rows in ctx->d_rs_in instead).  Each part copies its own slice in on its own stream
@@ -587,6 +605,7 @@ int RunEncode(lyra_b200_ctx* ctx, const CodecCall& c) {
     if ((rc = LaunchEncoderNets(ctx, p, skip, pcm16, ctx->d_features, active))) return rc;
     if ((rc = LaunchQuantize(ctx, p.st, Rows(p, c.d_ids, active), c.words, ctx->d_features, c.num_bits, d.packets_out, nullptr, skip)))
       return rc;
+    if ((rc = LaunchCallStats(ctx, p, c, in, skip))) return rc;
     if (h.packets_out)
       CU(cudaMemcpyAsync(h.packets_out + (size_t)p.slot0 * pb, d.packets_out + (size_t)p.slot0 * pb, pb * (size_t)p.nslots, cudaMemcpyDeviceToHost, p.st));
     return LYRA_B200_OK;
@@ -620,6 +639,7 @@ int RunDecode(lyra_b200_ctx* ctx, const CodecCall& c) {
       if (h.flags) CU(cudaMemcpyAsync(h.flags + p.slot0, d.flags + p.slot0, (size_t)p.nslots, cudaMemcpyDeviceToHost, p.st));
     }
     if (rs && (rc = LaunchCodecResample(ctx, p.st, io, c.words, 1, pcm16, out))) return rc;
+    if ((rc = LaunchCallStats(ctx, p, c, out, d.received))) return rc;
     if (h.pcm_out)
       CU(cudaMemcpyAsync(h.pcm_out + (size_t)p.slot0 * hop, out + (size_t)p.slot0 * hop, sizeof(int16_t) * hop * (size_t)p.nslots,
                          cudaMemcpyDeviceToHost, p.st));
@@ -659,6 +679,7 @@ int RunDecodePlc(lyra_b200_ctx* ctx, const CodecCall& c) {
       return rc;
     if ((rc = LaunchNoiseUpdate(ctx, p.st, planned, kWords16k, false, ctx->d_model_pcm, ctx->d_feed, nullptr, nullptr))) return rc;
     if (rs && (rc = LaunchCodecResample(ctx, p.st, io, c.words, 1, pcm16, out))) return rc;
+    if ((rc = LaunchCallStats(ctx, p, c, out, ctx->d_plan))) return rc;
     if (h.pcm_out)
       CU(cudaMemcpyAsync(h.pcm_out + (size_t)p.slot0 * hop, out + (size_t)p.slot0 * hop, sizeof(int16_t) * hop * (size_t)p.nslots,
                          cudaMemcpyDeviceToHost, p.st));
@@ -824,7 +845,8 @@ int RunMaybeGraphed(lyra_b200_ctx* ctx, const lyra_b200_ctx::GraphKey& key, bool
 
 // Every fused codec call past its own pointer checks: role, bit count (also against the listed streams' own counts, from the host
 // mirror), tile map; the stream ids go to the device when the call's chain has a kernel indexed by stream id (the converters, the
-// noise estimators, the PLC kernels, the RVQ kernels while some stream of the role has its own bit count).  A host-buffer call runs on the
+// noise estimators, the PLC kernels, the RVQ kernels while some stream of the role has its own bit count, CallStatsKernel while
+// statistics are on).  A host-buffer call runs on the
 // context's staging buffers, a call without a flag buffer on the context's, and only the dense host-buffer encode / decode may
 // replay a graph.  A host-buffer call returns when its results are in the caller's buffers; a *_device twin never waits.
 int RunCodecCall(lyra_b200_ctx* ctx, CodecCall c) {
@@ -841,7 +863,7 @@ int RunCodecCall(lyra_b200_ctx* ctx, CodecCall c) {
       return LYRA_B200_EINVAL;
     }
   }
-  const bool by_id = Converts(ctx) || (c.kind != kEncode && c.kind != kDecode) || ctx->own_words[r];
+  const bool by_id = Converts(ctx) || (c.kind != kEncode && c.kind != kDecode) || ctx->own_words[r] || ctx->stats_on;
   int rc = PrepareMap(ctx, c.ids, c.n);
   if (rc || (by_id && (rc = UploadIds(ctx, c.ids, c.n, &c.d_ids)))) return rc;
   const bool host = c.host.packets_in || c.host.packets_out;
@@ -862,9 +884,9 @@ int RunCodecCall(lyra_b200_ctx* ctx, CodecCall c) {
   const CodecCall::Io& h = c.host;
   const lyra_b200_ctx::GraphKey key =
       encoder ? lyra_b200_ctx::GraphKey{kEncode, c.n, c.num_bits, 0, ctx->nsplit, h.pcm_in, h.packets_out, nullptr, ctx->rate_override,
-                                        ctx->own_words[r] != 0}
+                                        ctx->own_words[r] != 0, ctx->stats_on}
               : lyra_b200_ctx::GraphKey{kDecode, c.n, c.num_bits, ctx->decoder_mode, ctx->nsplit, h.packets_in, h.received, h.pcm_out,
-                                        ctx->rate_override, ctx->own_words[r] != 0};
+                                        ctx->rate_override, ctx->own_words[r] != 0, ctx->stats_on};
   const bool graphed = host && (c.kind == kEncode || c.kind == kDecode) && c.ids == nullptr && ctx->map_dense_n == c.n;
   if ((rc = RunMaybeGraphed(ctx, key, graphed, [&]() {
          return encoder ? RunEncode(ctx, c) : c.kind == kDecodePlc ? RunDecodePlc(ctx, c) : RunDecode(ctx, c);
@@ -940,6 +962,10 @@ const char* RecordProblem(const lyra_b200_ctx* ctx, const uint8_t* rec) {
     if (check == lyra_b200_ctx::kCheckStreamBits && RecordWord(rec, w0) != 0 && !StreamBitsOk(ctx, (int32_t)RecordWord(rec, w0)))
       return "stream bit count is not a multiple of 4 in 4..184";
     if (check == lyra_b200_ctx::kCheckStreamDtx && RecordWord(rec, w0) > 1u) return "stream DTX word is not 0 or 1";
+    if (check == lyra_b200_ctx::kCheckStats &&
+        (RecordWord(rec, w0 + 2 * kStatLevel) > (uint32_t)kStatsLevels || RecordWord(rec, w0 + 2 * kStatLevel + 1) != 0 ||
+         RecordWord(rec, w0 + 2 * kStatPrevReceived) > 1u || RecordWord(rec, w0 + 2 * kStatPrevReceived + 1) != 0))
+      return "call statistics: level above 127 or event state not 0 or 1";
   }
   return nullptr;
 }
@@ -1216,6 +1242,19 @@ int lyra_b200_create_ex(const char* model_dir, int device, int max_streams, int 
     ok = ok && DevStreamState(ctx, &ctx->d_codec_rs_pos[d], 2, nullptr, d == 0 ? kStateCodecRs0 : kStateCodecRs1,
                               lyra_b200_ctx::kCheckResamplerPos);
   }
+  // the call statistics per role (lyra_b200_set_stats): LEVEL 127 and "last run hop received" at creation and after reset
+  // (registered after the network entries and before the per-stream words, which stay the last words of a record)
+  unsigned long long stats0[kStatsWords] = {};
+  stats0[kStatLevel] = kStatsLevels;
+  stats0[kStatPrevReceived] = 1;
+  for (int r = 0; r < 2; ++r)
+    if (roles & (r == 0 ? LYRA_B200_ROLE_ENCODER : LYRA_B200_ROLE_DECODER))
+      ok = ok && DevStreamState(ctx, &ctx->d_stats[r], (size_t)kStatsWords, stats0, kStatePlain, lyra_b200_ctx::kCheckStats);
+  double levels[kStatsLevels + 1] = {};
+  for (int k = 0; k < kStatsLevels; ++k) levels[k] = 1073741824.0 * std::pow(10.0, -(k + 0.5) / 10.0);
+  ok = ok && DevAlloc(ctx, &ctx->d_stats_levels, (size_t)kStatsLevels + 1) &&
+       cudaMemcpy(ctx->d_stats_levels, levels, sizeof(levels), cudaMemcpyHostToDevice) == cudaSuccess;
+  ok = ok && DevAlloc(ctx, &ctx->d_stats_out, P * kStatsWords);
   // the stream's DTX word (lyra_b200_set_stream_dtx, encoder role): 0, DTX on, at creation and after reset; then its own bit
   // count per role (lyra_b200_set_stream_bits): 0, the call's, at creation and after reset
   // (registered before the rate word, which stays the last word of a record)
@@ -1506,6 +1545,45 @@ int lyra_b200_set_active_mask(lyra_b200_ctx* ctx, const uint8_t* d_active) {
   if (!ctx) return LYRA_B200_EINVAL;
   ctx->d_active = d_active;          // read by the kernels of later *_device codec calls, in stream order
   return LYRA_B200_OK;
+}
+
+int lyra_b200_set_stats(lyra_b200_ctx* ctx, int enable) {
+  if (!ctx) return LYRA_B200_EINVAL;
+  ctx->stats_on = enable != 0;       // read by the host when later codec calls are issued
+  return LYRA_B200_OK;
+}
+
+int lyra_b200_read_stats(lyra_b200_ctx* ctx, int role, const int32_t* stream_ids, int n, uint64_t* stats, int clear) {
+  if (!ctx) return LYRA_B200_EINVAL;
+  if (!stats) { ctx->err = "stats is required"; return LYRA_B200_EINVAL; }
+  ENTER(0);
+  const int r = BitsRole(ctx, role);
+  if (r < 0) return LYRA_B200_EINVAL;
+  const int* d_ids = nullptr;
+  int rc = CheckIds(ctx, stream_ids, n, true);
+  if (rc || (rc = UploadIds(ctx, stream_ids, n, &d_ids))) return rc;
+  const dim3 grid((unsigned)((n * kStatsWords + 255) / 256));
+  // repeated ids: every read before any clear
+  if ((rc = LAUNCH(kNoProf, StatsReadKernel, grid, dim3(256), (size_t)0, ctx->stream, ctx->d_stats[r], d_ids, n, ctx->d_stats_out,
+                   clear && !d_ids ? 1 : 0)))
+    return rc;
+  if (clear && d_ids &&
+      (rc = LAUNCH(kNoProf, StatsReadKernel, grid, dim3(256), (size_t)0, ctx->stream, ctx->d_stats[r], d_ids, n, nullptr, 1)))
+    return rc;
+  CU(cudaMemcpyAsync(stats, ctx->d_stats_out, sizeof(uint64_t) * kStatsWords * (size_t)n, cudaMemcpyDeviceToHost, ctx->stream));
+  CU(SyncStream(ctx));
+  return LYRA_B200_OK;
+}
+
+int lyra_b200_read_stats_device(lyra_b200_ctx* ctx, int role, int n, uint64_t* d_stats, int clear) {
+  if (!ctx) return LYRA_B200_EINVAL;
+  if (!d_stats) { ctx->err = "d_stats is required"; return LYRA_B200_EINVAL; }
+  ENTER(0);
+  const int r = BitsRole(ctx, role);
+  if (r < 0) return LYRA_B200_EINVAL;
+  if (int rc = CheckIds(ctx, nullptr, n, false)) return rc;
+  return LAUNCH(kNoProf, StatsReadKernel, dim3((unsigned)((n * kStatsWords + 255) / 256)), dim3(256), (size_t)0, ctx->stream,
+                ctx->d_stats[r], nullptr, n, reinterpret_cast<unsigned long long*>(d_stats), clear ? 1 : 0);
 }
 
 int lyra_b200_synchronize(lyra_b200_ctx* ctx) {

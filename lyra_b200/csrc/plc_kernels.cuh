@@ -250,4 +250,92 @@ ResampleKernel(const uint8_t* __restrict__ blob, ResamplerParams P, int pair, in
   }
 }
 
+// ------------------------------------------------------------------------------------------------
+// Per-stream call statistics (lyra_b200_set_stats / _read_stats).  One entry per role, row-major, kStatsWords u64 per stream:
+// the public words LYRA_B200_STAT_* (0..6) and word kStatPrevReceived, whether the stream's last run hop was received (decoder
+// role; initially 1, so a first run hop that is not received is a concealment event).
+constexpr int kStatsWords = 8;
+constexpr int kStatHops = 0, kStatSatOut = 1, kStatEnergy = 2, kStatLevel = 3, kStatEmpty = 4, kStatBits = 5, kStatReceived = 4,
+              kStatCnHops = 5, kStatEvents = 6, kStatPrevReceived = 7;
+constexpr int kStatsLevels = 127;                 // RFC 6464 levels 1..127 (-dBov); the host's threshold table has 128 entries
+constexpr int kStatsThreads = 256;                // one warp per row
+constexpr int kStatsRowsPerBlock = kStatsThreads / 32;
+// what the event source of CallStatsKernel is: encode (none), encode_dtx (the DTX flags, 1 = empty packet), decode /
+// decode_track_noise (the received bytes, nullptr = every packet arrived), decode_plc (the plan bytes of PlcPlanKernel)
+enum StatsSource { kStatsEncode = 0, kStatsEncodeDtx = 1, kStatsDecode = 2, kStatsDecodePlc = 3 };
+
+// sum of the squares of the two int16 samples in w (each square <= 2^30, so the pair fits 32 bits)
+__device__ __forceinline__ uint32_t SquarePair(uint32_t w) {
+  const int lo = (int)(int16_t)(w & 0xffffu), hi = (int)(int16_t)(w >> 16);
+  return (uint32_t)(lo * lo) + (uint32_t)(hi * hi);
+}
+
+// One warp per row of the call: the first rate / 50 samples of the row (rows row_stride samples apart) -> their exact sum of
+// squares, with 16-byte loads over the row's 16-byte aligned middle (the ABI promises 2-byte alignment only) and a warp
+// shuffle reduction; then lane 0 updates the statistics of the row's stream.  levels: the 128 host-computed thresholds
+// t_k = 2^30 10^(-(k + 0.5) / 10), k < 127, and 0.  A slot that sits out counts kStatSatOut only and its row and event byte are
+// not read.  bits: the call's num_bits (encoder role).
+__global__ void __launch_bounds__(kStatsThreads)
+CallStatsKernel(const __grid_constant__ RowIo io, const __grid_constant__ StreamWords words, const int16_t* __restrict__ pcm,
+                int row_stride, int source, const uint8_t* __restrict__ events, int num_bits, const double* __restrict__ levels,
+                unsigned long long* __restrict__ stats) {
+  const int lane = (int)threadIdx.x % 32;
+  const int row = (int)blockIdx.x * kStatsRowsPerBlock + (int)threadIdx.x / 32, slot = io.slot0 + row;
+  if (row >= io.slots) return;
+  const int stream = io.Stream(slot);
+  unsigned long long* st = stats + (size_t)stream * kStatsWords;
+  if (io.SatOut(slot)) {
+    if (lane == 0) st[kStatSatOut] += 1;
+    return;
+  }
+  const int samples = words.Rate(stream) / 50;
+  const int16_t* x = pcm + (size_t)slot * row_stride;
+  int head = (int)((16u - ((unsigned)(uintptr_t)x & 15u)) & 15u) / 2;
+  head = head < samples ? head : samples;
+  const int vecs = (samples - head) / 8;
+  const uint4* xv = reinterpret_cast<const uint4*>(x + head);
+  unsigned long long sq = 0;
+  if (lane < head) sq += (unsigned long long)((int)x[lane] * (int)x[lane]);
+  for (int i = lane; i < vecs; i += 32) {
+    const uint4 v = xv[i];
+    sq += (unsigned long long)SquarePair(v.x) + SquarePair(v.y) + (unsigned long long)SquarePair(v.z) + SquarePair(v.w);
+  }
+  for (int i = head + vecs * 8 + lane; i < samples; i += 32) sq += (unsigned long long)((int)x[i] * (int)x[i]);
+#pragma unroll
+  for (int m = 16; m >= 1; m >>= 1) sq += __shfl_xor_sync(0xffffffffu, sq, m);
+  const double msq = __ddiv_rn((double)sq, (double)samples);
+  int level = 0;
+  for (int k = lane; k < kStatsLevels; k += 32) level += levels[k] > msq ? 1 : 0;
+#pragma unroll
+  for (int m = 16; m >= 1; m >>= 1) level += __shfl_xor_sync(0xffffffffu, level, m);
+  if (lane != 0) return;
+  st[kStatHops] += 1;
+  st[kStatEnergy] += sq / (unsigned long long)samples;
+  st[kStatLevel] = (unsigned long long)level;
+  if (source == kStatsEncode || source == kStatsEncodeDtx) {
+    if (source == kStatsEncodeDtx && events[slot]) st[kStatEmpty] += 1;
+    else st[kStatBits] += (unsigned long long)(words.Stages(stream, num_bits / kRvqBitsPerStage) * kRvqBitsPerStage);
+    return;
+  }
+  const int e = events ? events[slot] : 1;
+  const bool received = source == kStatsDecodePlc ? (e & 4) != 0 : e != 0;
+  if (received) st[kStatReceived] += 1;
+  if (source == kStatsDecodePlc && (e & 2)) st[kStatCnHops] += 1;
+  if (!received && st[kStatPrevReceived]) st[kStatEvents] += 1;
+  st[kStatPrevReceived] = received ? 1ull : 0ull;
+}
+
+// lyra_b200_read_stats(_device): out[k] (nullptr: no read) <- the public words of stream ids[k] (ids nullptr: k) in the entry
+// `stats`, word kStatPrevReceived read as 0; with clear the counters and the energy are zeroed after the read (LEVEL and the
+// private word stay).  A read with repeated ids and clear runs as a read launch followed by a clear launch.
+__global__ void __launch_bounds__(256)
+StatsReadKernel(unsigned long long* __restrict__ stats, const int* __restrict__ ids, int n, unsigned long long* __restrict__ out,
+                int clear) {
+  const int g = (int)(blockIdx.x * blockDim.x + threadIdx.x), k = g / kStatsWords, w = g % kStatsWords;
+  if (k >= n) return;
+  unsigned long long* v = stats + (size_t)(ids ? ids[k] : k) * kStatsWords + w;
+  if (out) out[g] = w == kStatPrevReceived ? 0ull : *v;
+  if (clear && w != kStatLevel && w != kStatPrevReceived) *v = 0ull;
+}
+
 }  // namespace lyra_b200

@@ -26,16 +26,21 @@ run in one process so that clock and thermal drift hit them alike:
   mask-tiles         16k with the tiles alternating hop by hop: the even tiles run on even hops, the odd tiles on odd hops (a
                      server that ticks every 10 ms and staggers the 20 ms hop phase of its calls tile by tile);
   mask-lanes         16k with a rotating quarter of the lanes of every tile sitting out (lanes 2k, 2k + 1 on hops i = k mod 4),
-                     every stream aligned with the first lane of its tile every 25 hops (lyra_b200_align_streams).
+                     every stream aligned with the first lane of its tile every 25 hops (lyra_b200_align_streams);
+  stats              shorthand for the four configurations below, alternated like any others:
+  stats-off-16k,     16k and 48k with the per-stream call statistics off (the default) and on (lyra_b200_set_stats: one
+  stats-on-16k,      CallStatsKernel launch per sub-batch of every codec call), to compare pairwise.
+  stats-off-48k,
+  stats-on-48k
 Frames/s counts every stream's hops, also those it sits out; the mask configurations also report the active fraction.
 The dtx configurations also report the fraction of DTX hops over the timed runs.
 Prints one line per run, then every configuration's median, spread and ratio to the first configuration, the card's name,
 power limit and median SM clock over the timed runs, and a JSON line.  --profile-hops adds a torch.profiler pass per
-configuration, separate from the timed runs: the mean device time per launch of ResampleKernel, RvqEncodeKernel and
-RvqDecodeKernel.
+configuration, separate from the timed runs: the mean device time per launch of ResampleKernel, RvqEncodeKernel,
+RvqDecodeKernel and CallStatsKernel.
 
   python tools/schedule_bench.py [--configs 16k,48k,8k,mixed,split,bits-184,bits-mixed,bits-split,mixed-counters,aligned-counters,
-                                            dtx,dtx-mixed,dtx-split,dtx-off,mask-ones,mask-tiles,mask-lanes]
+                                            dtx,dtx-mixed,dtx-split,dtx-off,mask-ones,mask-tiles,mask-lanes,stats]
                                  [--streams 4096]
                                  [--hops 200] [--runs 5]
 """
@@ -56,8 +61,10 @@ import duplex_schedule as ds  # noqa: E402
 RATES = (8000, 16000, 32000, 48000)
 BIT_RATES = (64, 120, 184)
 CONFIGS = ("16k", "8k", "32k", "48k", "mixed", "split", "bits-184", "bits-mixed", "bits-split", "mixed-counters", "aligned-counters",
-           "dtx", "dtx-mixed", "dtx-split", "dtx-off", "mask-ones", "mask-tiles", "mask-lanes")
-PROFILED = ("ResampleKernel", "RvqEncodeKernel", "RvqDecodeKernel")
+           "dtx", "dtx-mixed", "dtx-split", "dtx-off", "mask-ones", "mask-tiles", "mask-lanes", "stats-off-16k", "stats-on-16k",
+           "stats-off-48k", "stats-on-48k")
+STATS = ("stats-off-16k", "stats-on-16k", "stats-off-48k", "stats-on-48k")
+PROFILED = ("ResampleKernel", "RvqEncodeKernel", "RvqDecodeKernel", "CallStatsKernel")
 # active-mask patterns of the mask-* configurations (rows of all groups, 8-stream tiles), applied hop by hop in turn
 MASKS = {
     "mask-ones": lambda n: [np.ones(n, np.uint8)],
@@ -97,6 +104,13 @@ def make(name, args):
                            stream_bits=stream_bits, dtx=dtx, mask=mask, realign=realign)
 
     n, g = args.streams, args.groups
+    if name in STATS:
+        s = sched(n, g, int(name[-3:-1]) * 1000)
+        if name.startswith("stats-on"):
+            for enc, dec, _, _ in s.groups:
+                enc.set_stats(1)
+                dec.set_stats(1)
+        return [s]
     if name.startswith("mask-"):
         return [sched(n, g, mask=MASKS[name](n), realign=25 if name == "mask-lanes" else 0)]
     if name in ("dtx", "dtx-mixed", "dtx-off"):
@@ -148,7 +162,7 @@ def main():
     ap.add_argument("--decoder-mode", default="tensor", choices=["exact", "tensor"])
     ap.add_argument("--profile-hops", type=int, default=0, help="hops of the per-kernel profiler pass (0: none)")
     args = ap.parse_args()
-    names = args.configs.split(",")
+    names = [k for c in args.configs.split(",") for k in (STATS if c == "stats" else (c,))]
     bad = [k for k in names if k not in CONFIGS]
     if bad:
         ap.error("unknown configuration %s" % ", ".join(bad))
